@@ -1,9 +1,10 @@
 #!/usr/bin/env python
-"""bench.py -- benchmarks of the NeRSemble render hot path on B200 (one JSON line on rank 0).
+"""bench.py -- benchmarks of the NeRSemble render hot path on H100 (one JSON line on rank 0).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--config 2|2occ|3|4|5] [--scaling strong|weak] [--impl reference]
+                    [--dump-outputs DIR]
 
-Default (what the driver runs): BASELINE.json config 2 -- 4096 rays x 256 samples = 2^20 samples, 32-member hash
+Default: BASELINE.json config 2 -- 4096 rays x 256 samples = 2^20 samples, 32-member hash
 ensemble with full-size tables (16 levels x 2^19), T = 24, fused forward + alpha composite.
 
   value     device-resident inputs, ONE kernel launch per step: fixed-stride march -> fused field -> composite
@@ -18,6 +19,10 @@ ensemble with full-size tables (16 levels x 2^19), T = 24, fused forward + alpha
             per-pixel L2 < 1e-3); the run fails when it is exceeded.
   roofline  HBM: 16 384 algorithmic bytes per sample / time of the fused render kernel (CUDA events around its launch).
   cpu_baseline  the oracle port timed on the host cores on those 64 rays (1 warm-up + median of 5).
+
+--dump-outputs DIR (config 2): after the timed steps, the per-ray outputs of the last timed step (rgb, accumulation,
+depth, deformation, num_samples_per_ray; with strong scaling the all-gathered rgb of the whole batch) as DIR/<name>.npy, float32 (the sample counts float64).  Inputs and parameters
+are seeded, so two builds run with the same arguments can be compared output for output.
 
 Other configs (BASELINE.json configs[2..4]; `--config`): 2occ = config 2 with a seeded blob occupancy grid through the
 plugin sampler; 3 = full training step of the seq-30 recipe (jittered occupancy march + visibility pre-pass, six losses,
@@ -161,7 +166,7 @@ def peaks():
     if os.path.exists(p):
         j = json.load(open(p))
         return float(j["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3)"
 
 
 class ClockSampler(threading.Thread):
@@ -226,8 +231,8 @@ def cpu_oracle(S, o, d, times, repeats=5, mode="none"):
     P = oracle_field_params(S)
     Precision.mode = mode
     ts, te, ri = pl.fixed_samples(o, d, P.aabb, SAMPLES_PER_RAY, STEP, near=NEAR)
-    # thread count: the oracle is gather-bound torch code that does NOT scale to every hardware thread (r1: the same
-    # code gave 0.0007 .. 0.0089 M samples/s between boxes with torch.set_num_threads(os.cpu_count())); calibrate on
+    # thread count: the oracle is gather-bound torch code that does NOT scale to every hardware thread (with
+    # torch.set_num_threads(os.cpu_count()) it can run many times slower than with fewer threads); calibrate on
     # 8 rays and keep the fastest setting -- `cores` reports what was used
     global _ORACLE_THREADS
     if "_ORACLE_THREADS" not in globals():
@@ -261,7 +266,7 @@ def run_reference(args):
         return
     S = synthetic_params()
     o, d, t = synthetic_rays(RAYS, 1000)
-    reps = max(1, min(args.steps, 5))
+    reps = max(1, args.steps)
     _, sec, threads, n = cpu_oracle(S, o[:PARITY_RAYS], d[:PARITY_RAYS], t[:PARITY_RAYS], repeats=reps)
     v = n / sec / 1e6
     sample = f"{PARITY_RAYS} rays x {SAMPLES_PER_RAY} samples ({n} samples) per step, full-size tables, oracle/pipeline.py torch CPU fp32; 1 warm-up + median of {reps}"
@@ -312,7 +317,7 @@ class Dist:
 
     def close(self):
         """End of the run.  N > 1: communicators that were captured into CUDA graphs made destroy_process_group() hang
-        (r2i: rank 0 had printed its line, then torchrun sat until the outer timeout), so the graphs are reset first and
+        (rank 0 had printed its line, then torchrun sat until an outer timeout), so the graphs are reset first and
         the process leaves through os._exit after a last barrier."""
         import torch
         for g in _GRAPHS:
@@ -375,6 +380,17 @@ def graphed(fn, dev):
         return fn, False
 
 
+def dump_outputs(dirname, out):
+    """Per-ray outputs of one render call as DIR/<name>.npy: float32, integer counts as float64 (a few hundred KB)."""
+    import numpy as np
+    os.makedirs(dirname, exist_ok=True)
+    for k in ("rgb", "accumulation", "depth", "deformation", "num_samples_per_ray"):
+        if k in out:
+            t = out[k].detach()
+            a = t.float().cpu().numpy() if t.is_floating_point() else t.double().cpu().numpy()
+            np.save(os.path.join(dirname, k + ".npy"), a)
+
+
 # ------------------------------------------------------------------------------------------------ config 2
 def run_config2(args, occ=False):
     import torch
@@ -401,6 +417,7 @@ def run_config2(args, occ=False):
     o_s, d_s, t_s = o_g[lo:hi].to(dev), d_g[lo:hi].to(dev), t_g[lo:hi].to(dev)
     o_w, d_w, t_w = [x.to(dev) for x in synthetic_rays(RAYS, 1000 + rank)]
     ev_field = []
+    last = {}       # the outputs of the latest render() call of the timed path (--dump-outputs)
 
     def render(o, d, t, time_field=False):
         """ONE launch: fixed-stride march -> fused field -> composite + depth clip (nsb_render_forward)."""
@@ -441,18 +458,24 @@ def run_config2(args, occ=False):
         def step_value():
             out = render(o_s, d_s, t_s)
             D.dist.all_gather_into_tensor(rgb_all, out["rgb"])      # balanced shards: 4096 % world == 0
+            last["out"] = out       # graph replays write into the buffers of the captured call
         assert RAYS % world == 0
         step_fn, was_graphed = graphed(step_value, dev)
     else:
-        step_fn, was_graphed = (lambda: render(o_w, d_w, t_w)), False
+        def step_value():
+            last["out"] = render(o_w, d_w, t_w)
+        step_fn, was_graphed = step_value, False
     for _ in range(W):
         step_fn()
     ms_value = timed(D, step_fn, K, sampler)
+    if args.dump_outputs and rank == 0:
+        # strong scaling: what every rank receives is the all-gathered RGB of the whole batch
+        dump_outputs(args.dump_outputs, {"rgb": rgb_all} if strong else last["out"])
     # fused field kernel alone (CUDA events around the launch, separate pass so that the events do not sit in the graph)
     for _ in range(2):
         render(o_s, d_s, t_s, time_field=False)
     D.barrier()
-    for _ in range(min(K, 10)):
+    for _ in range(K):
         render(o_s, d_s, t_s, time_field=True)
     D.barrier()
     field_ms = sum(a.elapsed_time(b) for a, b in ev_field) / len(ev_field)
@@ -518,12 +541,8 @@ def run_config2(args, occ=False):
         e2e_val = samples_e2e_total * K / (ms_e2e / 1e3) / 1e6
         field_samples = (hi - lo) * SAMPLES_PER_RAY
         achieved = ALG_BYTES_PER_SAMPLE * field_samples / (field_ms / 1e3) / 1e9
-        traffic = None
         from nersemble_b200 import ops as _ops
         kname = "render_kernel_tc" if _ops.USE_TCGEN05 else "render_kernel_ws"      # NSB_TCGEN05=0 selects the mma.sync role
-        tp = os.path.join(ROOT, "profiles", "traffic.json")
-        if os.path.exists(tp) and world == 1:
-            traffic = json.load(open(tp)).get(f"{kname}_dram_bytes_per_launch")
         line = {
             "metric": "M ray-samples/sec", "value": value, "unit": "M ray-samples/s", "n_gpus": world, "steps": K,
             "warmup": W, "ms_per_step": ms_value / K, "higher_is_better": True,
@@ -535,7 +554,7 @@ def run_config2(args, occ=False):
                        "parallelism": (f"rays sharded 1/{world} per GPU, per-ray RGB all-gathered (NCCL) inside the timed region"
                                        if strong else f"ray-sharded x{world} (no collective)"),
                        "cuda_graph": was_graphed,
-                       "l2": "806 MB of hash tables are gathered every step (>> 126 MB L2); no explicit flush"},
+                       "l2": "806 MB of hash tables are gathered every step (>> 50 MB L2); no explicit flush"},
             "e2e": {"value": e2e_val, "unit": "M ray-samples/s", "h2d_bytes_per_step": RAYS * 9 * 4 * (1 if strong or world == 1 else world),
                     "d2h_bytes_per_step": RAYS * 3 * 4 * (1 if strong or world == 1 else world),
                     "call": "NeRSembleNGPModel.get_outputs_for_camera_ray_bundle (occupancy sampler, nears/fars = 256 steps): "
@@ -543,9 +562,9 @@ def run_config2(args, occ=False):
                     "samples_per_step": samples_e2e_total, "ms_per_step": ms_e2e / K, "rgb_l2_max_vs_op_path": e2e_l2},
             "gpu_launches": 1 * K,
             "roofline": {"bound": "hbm", "kernel": f"nsb::{kname}<fixed march> (march + field + composite, one launch; deformation MLP on "
-                                                      + ("tcgen05/TMEM)" if _ops.USE_TCGEN05 else "mma.sync)"), "achieved": achieved,
+                                                      + ("wgmma)" if _ops.USE_TCGEN05 else "mma.sync)"), "achieved": achieved,
                          "peak": hbm_peak, "peak_source": peak_src, "unit": "GB/s", "frac": achieved / hbm_peak,
-                         "traffic": traffic, "kernel_ms": field_ms, "samples_per_launch": field_samples},
+                         "kernel_ms": field_ms, "samples_per_launch": field_samples},
             "clocks": sampler.summary(),
         }
         if ms_weak is not None:
@@ -575,10 +594,14 @@ def main():
     ap.add_argument("--ab", action="store_true", help="config 5, N > 1: also time all-reduce + full step vs the sharded optimiser in the same process")
     ap.add_argument("--no-shard", action="store_true", help="config 5: all-reduce the table gradient and step the full table on every rank")
     ap.add_argument("--overlap", action="store_true", help="config 5: issue the table-gradient all-reduce on a side stream as soon as the "
-                    "gradient is parked (measured SLOWER on 2 x B200: 30.8 vs 22.9 ms per step, see DESIGN.md section 6)")
+                    "gradient is parked")
     ap.add_argument("--height", type=int, default=1088)
     ap.add_argument("--width", type=int, default=1920)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="config 2: write the per-ray outputs of the last timed step to DIR/<name>.npy")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != "b200" or args.config not in ("2", "2occ")):
+        ap.error("--dump-outputs is supported for the CUDA path of config 2")
     if args.impl == "reference":
         return run_reference(args)
     if args.config in ("2", "2occ"):

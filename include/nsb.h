@@ -1,4 +1,4 @@
-/* nsb.h -- C ABI of libnsb.so: the B200-native NeRSemble render hot path.
+/* nsb.h -- C ABI of libnsb.so: the H100-native (sm_90a) NeRSemble render hot path.
  *
  * Plain C: raw DEVICE pointers, sizes, scalar hparams, an explicit cudaStream_t (passed as
  * void*).  No C++/torch types.  Every entry point returns 0 on success, non-zero on error;
@@ -66,15 +66,15 @@ typedef struct nsb_field_params {
     const float *deform_code_bias;  /* float [n_timesteps][2][128]: W_code(layer 0|4) . warp_code[t] + bias, fp32: the
                                        warp code only depends on the timestep, so its columns cost no tensor work
                                        (-26 % MACs).  Per-sample warp codes (component API): nsb_samples.sample_code_bias. */
-    const void *deform_packed_umma; /* optional: the same deformation weights as tcgen05 B operands -- 14 blocks per tile in
+    const void *deform_packed_umma; /* optional: the same deformation weights as wgmma B operands -- 14 blocks per tile in
                                        order of use (L0 | L1 x2 | L2 x2 | L3 x2 | L4 hidden x2, posenc | L5 x2 | heads x2), each
                                        [128 outputs x 64 inputs] fp16 (heads [16 x 64]) in K-major 8 x 16-byte core matrices
                                        (python: pack_deform_umma; nsb_deform_packed_umma_bytes()).  When set, the inference
-                                       kernels run the deformation MLP on tcgen05.mma with the accumulator in TMEM. */
+                                       kernels run the deformation MLP on wgmma.mma_async (sm_90a warpgroup MMA). */
     const void *frame_table;   /* optional, float2 [total_entries]: the tables blended with ONE timestep's member weights
                                   (nsb_blend_tables).  Only valid when EVERY sample of the call has that timestep (one
                                   camera frame): the gather then reads 8 B per corner from a 50 MB table that stays in L2
-                                  instead of a 128 B line from HBM.  Used by the tcgen05 inference kernels. */
+                                  instead of a 128 B line from HBM.  Used by the wgmma inference kernels. */
     const void *field_packed;  /* fp16 mlp_base + mlp_head weights in MMA-B fragment order */
     const void *warp_codes;    /* __half [n_timesteps][128]  (time_embedding_deformation) */
     const float *blend_codes;  /* float  [n_timesteps][32]   (time_embedding) */
@@ -271,6 +271,11 @@ typedef struct nsb_table_adam_args {
     float lr, beta1, beta2, eps, weight_decay;
     float bias_correction1;   /* 1 - beta1^step */
     float bias_correction2;   /* 1 - beta2^step */
+    /* The scalars of torch.optim.Adam's update, each formed in double precision on the host and rounded once to float,
+       as torch forms them: the table step is then bit-identical to torch's foreach Adam for the same gradient. */
+    float step_size;          /* lr / bias_correction1 */
+    float bias_correction2_sqrt; /* bias_correction2 ** 0.5 */
+    float one_minus_beta1, one_minus_beta2;
 } nsb_table_adam_args;
 int nsb_table_adam_step(const nsb_table_adam_args *args, void *stream);
 

@@ -1,4 +1,4 @@
-"""nersemble_b200 -- B200-native (sm_100a) render hot path for NeRSemble.
+"""nersemble_b200 -- H100-native (sm_90a) render hot path for NeRSemble.
 
 Python host code mirroring the reference's nerfstudio plugin surface
 (src/nersemble/nerfstudio/**) over a C-ABI CUDA library (libnsb.so, include/nsb.h).

@@ -63,7 +63,8 @@ class TableAdamArgs(C.Structure):
                 ("tables_half", C.c_void_p), ("grad", C.c_void_p), ("g_rank1", C.c_void_p), ("cw_slots", C.c_void_p),
                 ("n_slots", C.c_int32), ("grad_scale", C.c_float), ("lr", C.c_float), ("beta1", C.c_float),
                 ("beta2", C.c_float), ("eps", C.c_float), ("weight_decay", C.c_float), ("bias_correction1", C.c_float),
-                ("bias_correction2", C.c_float)]
+                ("bias_correction2", C.c_float), ("step_size", C.c_float), ("bias_correction2_sqrt", C.c_float),
+                ("one_minus_beta1", C.c_float), ("one_minus_beta2", C.c_float)]
 
 
 class LossArgs(C.Structure):

@@ -1,4 +1,4 @@
-// Backward of the density/colour MLPs and of the hash ensemble (training), sm_100a.
+// Backward of the density/colour MLPs and of the hash ensemble (training), sm_90a.
 //
 // Replaces the autograd of (reference, relative to /root/reference/src/nersemble/nerfstudio/):
 //   fields/nersemble_nerfacto_field.py:285-293,377   tcnn mlp_base / mlp_head backward, trunc_exp backward
@@ -13,7 +13,7 @@
 //     movmatrix, accumulated into a per-CTA fp32 shared-memory copy, flushed once with global atomics.
 //   Deltas are fp16 MMA operands -> a loss scale keeps them in range (tcnn does the same, x128).
 // hash_bwd_kernel: one warp per sample, lane (g,q) = (corner, 8-member group) exactly like the forward
-//   gather; per level one LDG.256 (values, for the time-code gradient) and four 16-byte vector reductions
+//   gather; per level one 32-byte load (values, for the time-code gradient) and four 16-byte vector reductions
 //   (red.global.add.v4.f32) into the fp32 gradient line of the table entry.
 #include <algorithm>
 
@@ -631,7 +631,7 @@ extern "C" int nsb_field_backward(const nsb_field_params *params, const nsb_fiel
         int dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&g_bwd_sms, cudaDevAttrMultiProcessorCount, dev);
-        if (g_bwd_sms <= 0) g_bwd_sms = 148;
+        if (g_bwd_sms <= 0) g_bwd_sms = 132;
     }
     cudaStream_t st = (cudaStream_t)stream;
     FieldBwdKArgs K;

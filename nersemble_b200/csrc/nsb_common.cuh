@@ -1,4 +1,4 @@
-// Shared device helpers for libnsb (sm_100a).
+// Shared device helpers for libnsb (sm_90a).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -51,15 +51,15 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t *bar, uint32_t parity) {
     return done != 0;
 }
 // Spin with back-off: a waiting warp must not burn issue slots the gather warps need
-// (ncu r1a: 26% of all issued instructions were TRYWAIT/YIELD/BRA of the idle producer).
+// (an idle producer spinning without sleep takes a large share of the issued instructions).
 #ifndef NSB_SPIN_LIMIT
 #define NSB_SPIN_LIMIT (1u << 27)   // ~several seconds: a protocol bug traps instead of hanging the GPU
 #endif
 template <int SLEEP_NS>
 __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
 #ifdef NSB_NO_SPIN_GUARD
-    // The forward kernel opts out: the counter costs a live register at every wait site (measured: 56 -> 320 B of
-    // spills, 2.6 -> 3.2 ms).  The backward kernels keep the guard.
+    // The forward kernel opts out: the counter costs a live register at every wait site, and with it spills.  The
+    // backward kernels keep the guard.
     while (!mbar_try_wait(bar, parity)) {
         if (SLEEP_NS > 0) __nanosleep(SLEEP_NS);
     }

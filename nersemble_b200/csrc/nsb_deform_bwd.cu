@@ -1,4 +1,4 @@
-// Backward of the SE(3) deformation field (training), sm_100a.
+// Backward of the SE(3) deformation field (training), sm_90a.
 //
 // Replaces the autograd of (reference, relative to /root/reference/src/nersemble/):
 //   nerfstudio/field_components/deformation_field.py:77-116,148-166   mlp_stem / mlp_r / mlp_v, offsets
@@ -177,7 +177,7 @@ __device__ __forceinline__ int enc_ref_col(int kp) {
 
 // ---------------------------------------------------------------------------------------------
 // Weight-gradient accumulation.  First version: every tile added its dW block to the fp32 gradient with atomicAdd --
-// 127 K atomics per 128-row tile, 1.8 G per step on ~126 K hot addresses: the kernel's bottleneck (9.1 ms).  Now each
+// 127 K atomics per 128-row tile, 1.8 G per step on ~126 K hot addresses: the kernel's bottleneck.  Now each
 // CTA owns a private fp32 accumulator in FRAGMENT order (workspace [cta][kScrF4] float4): a lane adds its MMA
 // accumulators to its own float4 slots -- coalesced 512 B per warp access, no atomics, L2-resident (0.5 MB per CTA) --
 // and deform_dw_reduce_kernel sums the CTAs' accumulators into the reference layout once at the end.
@@ -278,7 +278,7 @@ __global__ void __launch_bounds__(256) deform_dw_reduce_kernel(const __grid_cons
 // 16 warps, two roles that only meet at the per-layer barriers:
 //   CHAIN warps 0-7  : rows 16w..16w+15 -- SE(3) backward, delta chain through the transposed weights (ring), staging
 //   DW    warps 8-15 : output block ob = w - 8 of every weight gradient (tile-wide contraction), bias sums
-// (One role per warp doubled the resident warps: the r1e capture of the 8-warp version showed 22 % issue-active at
+// (One role per warp doubled the resident warps: the 8-warp version was latency-bound at
 //  12.5 % occupancy, the dX chain and the dW contraction of a layer are independent once D / X are staged.)
 constexpr int kDbThreads = 512;
 __global__ void __launch_bounds__(kDbThreads, 1) deform_bwd_kernel(const __grid_constant__ DeformBwdKArgs K) {
@@ -604,7 +604,7 @@ static int db_sms() {
         int dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&g_db_sms, cudaDevAttrMultiProcessorCount, dev);
-        if (g_db_sms <= 0) g_db_sms = 148;
+        if (g_db_sms <= 0) g_db_sms = 132;
     }
     return g_db_sms;
 }

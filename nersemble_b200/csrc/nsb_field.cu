@@ -1,4 +1,4 @@
-// Fused per-sample field evaluation for sm_100a:
+// Fused per-sample field evaluation for sm_90a:
 //   windowed posenc + warp code -> SE(3) deformation MLP (tensor cores) -> warp ->
 //   32-member hash-ensemble gather + time-latent blend (HBM-bound) -> density MLP -> colour MLP.
 //
@@ -69,12 +69,12 @@ __device__ __forceinline__ void se3_apply(const float p[3], const float r[3], co
 }
 
 // ===========================================================================================
-// v2: warp-specialised persistent kernel, 1 CTA per SM (profiles/r1: with every warp doing every stage the
-// gather is latency-bound on the number of gathering warps and cannot overlap the deformation phase).
-//   4 TENSOR warps (120 regs): deformation MLP of tile i+1 (32 rows each, B fragments reused by two
-//     m-tiles), then density+colour MLPs of tile i.  Tensor warp 0 lane 0 also refills the weight ring.
-//   24 GATHER warps (64 regs): nothing but the hash-ensemble gather; rows of a tile are claimed
-//     dynamically; each warp keeps 2 m-tiles (2 x 2 LDG.256) in flight.
+// v2: warp-specialised persistent kernel, 1 CTA per SM (with every warp doing every stage the gather is
+// latency-bound on the number of gathering warps and cannot overlap the deformation phase).
+//   8 TENSOR warps: deformation MLP of tile i+1 (16 rows each), then density+colour MLPs of tile i.  Tensor warp 0
+//     lane 0 also refills the weight ring.
+//   GATHER warps: nothing but the hash-ensemble gather; rows of a tile are claimed dynamically; each warp keeps
+//     2 m-tiles (2 x 2 x 32 B per lane) in flight.
 // Hand-off through shared memory, double-buffered by tile parity, two mbarrier arrays:
 //   xs_full[b]   tensor -> gather : warped positions of tile i are in sm.xs[b]
 //   feat_full[b] gather -> tensor : blended features of tile i are in sm.feat[b]
@@ -87,21 +87,28 @@ __device__ __forceinline__ void se3_apply(const float p[3], const float r[3], co
 constexpr int kMT = NSB_WS_MT;                    // m-tiles (16 rows) per tensor warp
 constexpr int kTRows = 16 * kMT;                  // rows per tensor warp
 constexpr int kTensorWarps = NSB_TILE / kTRows;   // 8 (kMT=1) or 4 (kMT=2)
-constexpr int kGatherWarps = 28 - kTensorWarps;   // 20 or 24: 28 warps = 7 warpgroups
+#ifndef NSB_GATHER_WARPS
+#define NSB_GATHER_WARPS 8
+#endif
+constexpr int kGatherWarps = NSB_GATHER_WARPS;    // multiple of 4: setmaxnreg works on warpgroups
 constexpr int kThreadsWS = (kTensorWarps + kGatherWarps) * 32;
-// Register budget: 896 threads are launched with 72 registers each (64512 of the SM's 65536).
-// setmaxnreg can only move registers WITHIN the CTA's allocation (inc blocks until a dec released
+// Register budget: the kernels are launched with kLaunchRegs registers per thread (the SM's 65536 over the CTA's threads,
+// in units of 8).  setmaxnreg can only move registers WITHIN the CTA's allocation (inc blocks until a dec released
 // enough -- an inc that exceeds the pool hangs the kernel), so
-//   kTensorWarps*32*kTensorRegs + kGatherWarps*32*kGatherRegs <= 64512.
+//   kTensorWarps*32*kTensorRegs + kGatherWarps*32*kGatherRegs <= kThreadsWS*kLaunchRegs.
+// 16 warps (128 registers at launch): the gather role gets 120 and the tensor role 136.  With more gather warps (and so
+// fewer registers per thread) sm_90 ptxas spills in the gather role's sample loop, and the wgmma tensor role spills below
+// 104 registers (tools/spill_report.py).
+constexpr int kLaunchRegs = (65536 / kThreadsWS) & ~7;
 #ifndef NSB_GATHER_REGS
-#define NSB_GATHER_REGS 64
+#define NSB_GATHER_REGS 120
 #endif
 #ifndef NSB_TENSOR_REGS
-#define NSB_TENSOR_REGS (NSB_WS_MT == 1 ? 80 : 120)
+#define NSB_TENSOR_REGS 136
 #endif
 constexpr int kGatherRegs = NSB_GATHER_REGS;
 constexpr int kTensorRegs = NSB_TENSOR_REGS;
-static_assert(kTensorWarps * 32 * kTensorRegs + kGatherWarps * 32 * kGatherRegs <= kThreadsWS * 72, "register pool");
+static_assert(kTensorWarps * 32 * kTensorRegs + kGatherWarps * 32 * kGatherRegs <= kThreadsWS * kLaunchRegs, "register pool");
 constexpr int kLaunchBoundWS = kThreadsWS;
 // Slab layout of deform_packed_tb: layers 0 and 4 without their 128 warp-code columns (those enter as the
 // per-timestep bias deform_code_bias[t][0|1][128]).
@@ -308,19 +315,19 @@ __global__ void __launch_bounds__(kLaunchBoundWS, 1) field_kernel_ws(const __gri
     constexpr bool FEAT_GIVEN = false;
     // NOTE: nothing is computed ahead of the role split on purpose.  Values shared by both roles get registers that
     // suit the 88-register tensor role, and the 64-register gather role then pays for them with spills inside its
-    // sample loop (measured: 2.59 -> 2.77 ms).  Each role derives its loop bounds itself.
+    // sample loop.  Each role derives its loop bounds itself.
 
 #define NSB_N_SAMPLES A.S.n_samples
 #include "nsb_field_setup.inc"
     if (warp >= kTensorWarps) {
         // =============================== GATHER warps ===============================
-        if (kGatherRegs != 72) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kGatherRegs));
+        if (kGatherRegs != kLaunchRegs) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kGatherRegs));
 #include "nsb_field_gather_role.inc"
         return;
     }
 
     // =============================== TENSOR warps ===============================
-    if (kTensorRegs != 72) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kTensorRegs));
+    if (kTensorRegs != kLaunchRegs) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kTensorRegs));
 #include "nsb_field_tensor_role.inc"
 #undef NSB_N_SAMPLES
 }
@@ -337,32 +344,26 @@ __global__ void __launch_bounds__(kLaunchBoundWS, 1) field_kernel_ws_given(const
 #define NSB_N_SAMPLES A.S.n_samples
 #include "nsb_field_setup.inc"
     if (warp >= kTensorWarps) {
-        if (kGatherRegs != 72) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kGatherRegs));
+        if (kGatherRegs != kLaunchRegs) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kGatherRegs));
 #include "nsb_field_gather_role.inc"
         return;
     }
-    if (kTensorRegs != 72) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kTensorRegs));
+    if (kTensorRegs != kLaunchRegs) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kTensorRegs));
 #include "nsb_field_tensor_role.inc"
 #undef NSB_N_SAMPLES
 }
 
 // ===========================================================================================
-// tcgen05 variant of the inference kernels: the deformation MLP on the 5th-generation tensor cores (TMEM accumulator,
-// one issuing thread, weights read from shared memory once per 128-row tile) -- nsb_field_tensor_role_tc.inc.
-// The gather role is the unchanged include; only the tensor role and the shared-memory plan differ.
+// wgmma variant of the inference kernels ("tc" kernels): the deformation MLP as warpgroup MMAs (accumulator in
+// registers, weights read from shared memory by the tensor core once per 64-row half of a 128-row tile) --
+// nsb_field_tensor_role_tc.inc.  The gather role is the unchanged include; only the tensor role and the shared-memory
+// plan differ.
 // ===========================================================================================
-#ifndef NSB_TC_PAIR
-#define NSB_TC_PAIR 0       // 1: two tiles per pass over the weights (nsb_field_tensor_role_tc2.inc); 0: one tile (..._tc.inc)
-#endif
 #ifndef NSB_FRAME_GATHER_WARPS
-#define NSB_FRAME_GATHER_WARPS 8     // measured (2^20 samples): 20 warps 1.25 ms, 16: 1.24, 12: 1.21, 8: 1.14
+#define NSB_FRAME_GATHER_WARPS 8
 #endif
 constexpr int kFrameGatherWarps = NSB_FRAME_GATHER_WARPS;   // frame-table gather: how many of the gather warps do work
-#if NSB_TC_PAIR
-constexpr int kTcStages = 3, kTcBlocksPerTile = 14, kTcTmemCols = 256, kTcTiles = 2;
-#else
-constexpr int kTcStages = 4, kTcBlocksPerTile = 14, kTcTmemCols = 128, kTcTiles = 1;
-#endif
+constexpr int kTcStages = 4, kTcBlocksPerTile = 14;
 #ifdef NSB_TC_PROF
 __device__ unsigned long long g_tc_prof[8], g_tc_prof_k[8];
 #define KPROF(i) if (threadIdx.x == 0 && blockIdx.x == 3) g_tc_prof_k[i] = (unsigned long long)clock64();
@@ -370,28 +371,19 @@ __device__ unsigned long long g_tc_prof[8], g_tc_prof_k[8];
 #define KPROF(i)
 #endif
 #ifndef NSB_TC_SPLIT
-#define NSB_TC_SPLIT 1      // deformation (tcgen05) and density / colour MLPs (mma.sync) on separate warp groups
+#define NSB_TC_SPLIT 1      // deformation (wgmma) and density / colour MLPs (mma.sync) on separate warp groups
 #endif
 constexpr size_t kTcPackedBytes = 12 * 16384 + 2 * 2048;
 
 struct alignas(1024) SmemTC {
-    uint8_t wring[kTcStages][16384];        // weight blocks [128 n x 64 k] (heads: [16 x 64]) in UMMA core-matrix order
-#if NSB_TC_PAIR
-    uint8_t a_enc[2][16384];                // posenc A operand [128 rows x 64 k] of the pair's two tiles
-    uint8_t act[2][32768];                  // hidden activations A operand [128 rows x 128 k] of the two tiles
-#else
+    uint8_t wring[kTcStages][16384];        // weight blocks [128 n x 64 k] (heads: [16 x 64]) in core-matrix order
     uint8_t a_enc[16384];                   // posenc A operand [128 rows x 64 k]
-    uint8_t act[32768];                     // hidden activations A operand [128 rows x 128 k]
-#endif
+    uint8_t act[2][32768];                  // hidden activations A operand [128 rows x 128 k], ping-pong between layers
     uint4 field_w[kFieldPackedU4];
     alignas(16) float bias[kBiasFloats];
-#if NSB_TC_PAIR
-    uint64_t full[kTcStages], empty[kTcStages], acc_bar[2], f_done[2];
-#else
-    uint64_t full[kTcStages], empty[kTcStages], acc_bar, f_done[2];
-#endif
+    uint64_t full[kTcStages], empty[kTcStages], f_done[2];
     uint64_t xs_full[2], feat_full[2];
-    uint32_t tmem_base;
+    int row_ts[NSB_TILE];                   // timestep of each row of the tile in flight (its code-bias row)
     int tile_ctr[2];
     int64_t n_dyn;
     uint64_t sampler_done;
@@ -412,7 +404,6 @@ static_assert(sizeof(SmemTC) <= 227 * 1024, "shared memory plan");
         for (int i = tid; i < (int)(sizeof(sm.a_enc) / 16); i += kThreadsWS) reinterpret_cast<uint4 *>(&sm.a_enc)[i] = make_uint4(0u, 0u, 0u, 0u); \
         if (tid == 0) {                                                                                             \
             for (int s = 0; s < kTcStages; ++s) { mbar_init(&sm.full[s], 1); mbar_init(&sm.empty[s], 1); }         \
-            for (int t = 0; t < kTcTiles; ++t) mbar_init(reinterpret_cast<uint64_t *>(&sm.acc_bar) + t, 1);            \
             mbar_init(&sm.f_done[0], 4); mbar_init(&sm.f_done[1], 4);                                               \
             for (int b = 0; b < 2; ++b) {                                                                           \
                 mbar_init(&sm.xs_full[b], 4);                                                                       \
@@ -421,10 +412,7 @@ static_assert(sizeof(SmemTC) <= 227 * 1024, "shared memory plan");
             }                                                                                                       \
             mbar_fence_init();                                                                                      \
         }                                                                                                           \
-        if (warp == 0) tc::tmem_alloc(&sm.tmem_base, kTcTmemCols);                                                  \
-        tc::fence_before_sync();                                                                                    \
         __syncthreads();                                                                                            \
-        tc::fence_after_sync();                                                                                     \
     }
 
 // FRAME: the gather role reads the member-blended frame table (nsb_field_gather_role_frame.inc)
@@ -437,7 +425,7 @@ __global__ void __launch_bounds__(kLaunchBoundWS, 1) field_kernel_tc(const __gri
 #define NSB_N_SAMPLES A.S.n_samples
     NSB_TC_SETUP()
     if (warp >= kTensorWarps) {
-        if (kGatherRegs != 72) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kGatherRegs));
+        if (kGatherRegs != kLaunchRegs) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kGatherRegs));
         if constexpr (FRAME) {
 #include "nsb_field_gather_role_frame.inc"
         } else {
@@ -445,12 +433,8 @@ __global__ void __launch_bounds__(kLaunchBoundWS, 1) field_kernel_tc(const __gri
         }
         return;
     }
-    if (kTensorRegs != 72) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kTensorRegs));
-#if NSB_TC_PAIR
-#include "nsb_field_tensor_role_tc2.inc"
-#else
+    if (kTensorRegs != kLaunchRegs) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kTensorRegs));
 #include "nsb_field_tensor_role_tc.inc"
-#endif
 #undef NSB_N_SAMPLES
 }
 
@@ -467,11 +451,11 @@ __global__ void __launch_bounds__(kLaunchBoundWS, 1) field_kernel_ws_dyn(const _
 #define NSB_N_SAMPLES (*reinterpret_cast<const volatile int64_t *>(&sm.n_dyn))
 #include "nsb_field_setup.inc"
     if (warp >= kTensorWarps) {
-        if (kGatherRegs != 72) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kGatherRegs));
+        if (kGatherRegs != kLaunchRegs) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kGatherRegs));
 #include "nsb_field_gather_role.inc"
         return;
     }
-    if (kTensorRegs != 72) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kTensorRegs));
+    if (kTensorRegs != kLaunchRegs) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kTensorRegs));
 #include "nsb_field_tensor_role.inc"
 #undef NSB_N_SAMPLES
 }
@@ -571,8 +555,8 @@ __device__ NSB_RK_SAMPLER_ATTR void render_sampler_phase(const RenderKArgs &K) {
         if (SAMPLER != 2 && !(SAMPLER == 4 && K.sampler != 0)) K.hdr->status = 0;
     }
     if constexpr (SAMPLER == 4) {
-        // run-time choice between the fixed march and given samples in ONE binary (the tcgen05 render kernel): two
-        // instantiations were two draws of ptxas' allocation of the gather role, and the fixed-march draw ran 15 % slower
+        // run-time choice between the fixed march and given samples in ONE binary (the wgmma render kernel): two
+        // instantiations are two draws of ptxas' allocation of the gather role
         if (K.sampler == 0) {
             fixed_march_rays(K, warp, lane);
             if (tid == 0) {
@@ -694,12 +678,12 @@ __global__ void __launch_bounds__(kLaunchBoundWS, 1) render_kernel_ws(const __gr
     if (tid == 0) mbar_init(&sm.sampler_done, 1);                          // fenced + published by the setup below
 #include "nsb_field_setup.inc"
     if (warp >= kTensorWarps) {
-        if (kGatherRegs != 72) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kGatherRegs));
+        if (kGatherRegs != kLaunchRegs) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kGatherRegs));
         mbar_wait<200>(&sm.sampler_done, 0);                               // the sampler is done, sm.n_dyn is set
 #include "nsb_field_gather_role.inc"
         return;
     }
-    if (kTensorRegs != 72) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kTensorRegs));
+    if (kTensorRegs != kLaunchRegs) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kTensorRegs));
     render_sampler_phase<SAMPLER>(K);                                      // S (ends with a grid barrier)
     // hand-off through an mbarrier rather than a named barrier shared by the two roles: compute-sanitizer synccheck
     // reports a barrier that warps reach from two different instructions as divergent
@@ -711,7 +695,7 @@ __global__ void __launch_bounds__(kLaunchBoundWS, 1) render_kernel_ws(const __gr
     render_composite_phase<SAMPLER>(K);                                    // C
 }
 
-// render_kernel_ws with the deformation MLP on tcgen05 / TMEM (nsb_field_tensor_role_tc.inc); SAMPLER 0 or 2
+// render_kernel_ws with the deformation MLP on wgmma (nsb_field_tensor_role_tc.inc); SAMPLER 2 or 4
 template <int SAMPLER, bool FRAME>
 __global__ void __launch_bounds__(kLaunchBoundWS, 1) render_kernel_tc(const __grid_constant__ RenderKArgs K) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -725,7 +709,7 @@ __global__ void __launch_bounds__(kLaunchBoundWS, 1) render_kernel_tc(const __gr
     NSB_TC_SETUP()
     KPROF(1)
     if (warp >= kTensorWarps) {
-        if (kGatherRegs != 72) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kGatherRegs));
+        if (kGatherRegs != kLaunchRegs) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kGatherRegs));
         mbar_wait<200>(&sm.sampler_done, 0);
         if constexpr (FRAME) {
 #include "nsb_field_gather_role_frame.inc"
@@ -734,16 +718,12 @@ __global__ void __launch_bounds__(kLaunchBoundWS, 1) render_kernel_tc(const __gr
         }
         return;
     }
-    if (kTensorRegs != 72) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kTensorRegs));
+    if (kTensorRegs != kLaunchRegs) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kTensorRegs));
     render_sampler_phase<SAMPLER, SmemTC>(K);
     KPROF(2)
     if (tid == 0) mbar_arrive(&sm.sampler_done);
     {
-#if NSB_TC_PAIR
-#include "nsb_field_tensor_role_tc2.inc"
-#else
 #include "nsb_field_tensor_role_tc.inc"
-#endif
     }
 #undef NSB_N_SAMPLES
     KPROF(3)
@@ -799,7 +779,7 @@ static int num_sms() {
         int dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-        if (g_num_sms <= 0) g_num_sms = 148;
+        if (g_num_sms <= 0) g_num_sms = 132;
     }
     return g_num_sms;
 }
@@ -892,7 +872,7 @@ static int launch_field(const FieldArgs &A, cudaStream_t st) {
         return 1;
     }
     if (D && F && A.P.deform_packed_umma && !A.S.sample_code_bias && !(A.out.xs || A.out.deform_acts || A.out.deform_enc || A.out.corner_vals || A.out.feat))
-        return launch_field_tc<H>(A, st);       // inference with the deformation MLP on tcgen05 / TMEM
+        return launch_field_tc<H>(A, st);       // inference with the deformation MLP on wgmma
     return launch_field_ws<D, F, H>(A, st);
 }
 
@@ -964,7 +944,7 @@ extern "C" int nsb_hash_blend_forward(const nsb_field_params *params, const nsb_
 // -------------------------------------------------------------------------------------------
 // nsb_blend_tables: frame table = the 32 members of every table entry blended with ONE timestep's weights
 // (cw[m] = code[m] * cw_scale[m] + cw_bias[m], hash_ensemble.py:119-139), float2 per entry.  8 lanes per entry
-// (16 B = 4 members each), fp32 accumulation; one streaming pass over the tables (HBM-bound: 1 GB at ~6 TB/s).
+// (16 B = 4 members each), fp32 accumulation; one streaming pass over the tables (HBM-bound).
 // -------------------------------------------------------------------------------------------
 namespace nsb {
 __global__ void __launch_bounds__(256) blend_tables_kernel(const uint4 *__restrict__ tables, const float *__restrict__ code,
@@ -1038,9 +1018,8 @@ static int launch_render_tc(const RenderKArgs &K, cudaStream_t st) {
 template <bool D, int SAMPLER>
 static int launch_render(const RenderKArgs &K, cudaStream_t st) {
     if constexpr (D && SAMPLER != 1)
-        if (K.F.P.deform_packed_umma)       // every instantiation is its own draw of ptxas' allocation: measured (tools/
-            // render_time.py, 2^20 samples) <0> 2.35 ms, <4> (run-time sampler choice, fixed march as a call) 2.13 fixed /
-            // 2.18 given, <2> 2.02 given -> the fixed march runs the <4> binary, given samples the <2> binary
+        if (K.F.P.deform_packed_umma)       // every instantiation is its own draw of ptxas' allocation: the fixed march
+            // runs the <4> binary (run-time sampler choice, fixed march as a call), given samples the <2> binary
             return SAMPLER == 0 ? launch_render_tc<4>(K, st) : launch_render_tc<2>(K, st);
     const size_t smem = sizeof(SmemWS);
     static bool configured = false;

@@ -3,14 +3,13 @@
 #include "nsb_common.cuh"
 
 #ifndef NSB_PREFETCH_QUADS
-// Measured r1e (tools/quick_time.py, full / no-deform): 2.38 / 2.10 ms with the quad-ahead L2 prefetch vs 2.27 / 1.92 ms
-// without, zero spills in both builds.  More requests in flight do not help: the kernel sits at the memory system's
-// REQUEST throughput for this access pattern (38 G L2 requests/s + 26 G DRAM lines/s; tools/randgather.cu tops out at
-// 45 G random lines/s), and every prefetched line is requested twice.
+// Quad-ahead L2 prefetch (off by default): more requests in flight need not help when the kernel sits at the memory
+// system's REQUEST throughput for this access pattern (tools/randgather.cu measures the random-line rate), and every
+// prefetched line is requested twice.
 #define NSB_PREFETCH_QUADS 0
 #endif
 #ifndef NSB_STREAM_HASHED
-#define NSB_STREAM_HASHED 0   // measured r1e: 2.78 vs 2.27 ms with L1::no_allocate on the hashed levels (they DO hit in L1: 4 lanes share a sector pair, neighbouring samples share corners)
+#define NSB_STREAM_HASHED 0   // L1::no_allocate on the hashed levels (off: they DO hit in L1 -- 4 lanes share a sector pair, neighbouring samples share corners)
 #endif
 
 namespace nsb {
@@ -105,9 +104,8 @@ __device__ __forceinline__ float gather_blend(const nsb_field_params &P, float x
 // registers (no conversion instructions), B = the sample's blend weights (fp16, like the
 // reference: hash_ensemble.py:155 casts the code to half), fp32 accumulate.
 //   m-tile t: rows 0-7 = level 2t corners 0-7, rows 8-15 = level 2t+1 corners 0-7.
-//   lane (g,q) owns corner g of every level and loads bytes [32q,32q+32) of its two lines with one
-//   256-bit LDG each (LDG.E.256: 4 lanes cover a whole 128 B line, so every table line is ONE L2/DRAM
-//   request -- two 64 B half-line requests hit the DRAM access-rate limit, profiles/r1 notes);
+//   lane (g,q) owns corner g of every level and loads bytes [32q,32q+32) of its two lines (ldg256: the 4 lanes
+//   of a quad cover a whole 128 B line);
 //   k-step s uses words s and 4+s, i.e. k=2q,2q+1 <-> member 8q+s (f0,f1) and k=2q+8,2q+9 <->
 //   member 8q+4+s.  B[k][n] = cw[member(k)] * (feat(k)==n), n<2.
 //   C (lanes q==0): c0,c1 = (level 2t, corner g, f0/f1); c2,c3 = (level 2t+1, corner g, f0/f1).
@@ -142,9 +140,11 @@ struct GatherTile {
     float w[2];
 };
 
-// 256-bit read-only global load (sm_100+: LDG.E.256)
+// 32 bytes read-only from global memory as two LDG.128 (sm_90 has no 256-bit load).  The first load of a quad already
+// touches all four sectors of the 128 B line, so the second one finds the line in L1.
 __device__ __forceinline__ void ldg256(const void *p, uint32_t (&r)[8]) {
-    asm volatile("ld.global.nc.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
+    asm volatile("ld.global.nc.v4.b32 {%0,%1,%2,%3}, [%8];\n\t"
+                 "ld.global.nc.v4.b32 {%4,%5,%6,%7}, [%8+16];"
                  : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
                  : "l"(p));
 }
@@ -152,7 +152,8 @@ __device__ __forceinline__ void ldg256(const void *p, uint32_t (&r)[8]) {
 // same, streaming: the line is not allocated in L1.  Hashed (fine) levels have no reuse between samples, and keeping
 // them out of L1 leaves it to the dense levels' lines, the code rows and the stack.
 __device__ __forceinline__ void ldg256_stream(const void *p, uint32_t (&r)[8]) {
-    asm volatile("ld.global.nc.L1::no_allocate.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
+    asm volatile("ld.global.nc.L1::no_allocate.v4.b32 {%0,%1,%2,%3}, [%8];\n\t"
+                 "ld.global.nc.L1::no_allocate.v4.b32 {%4,%5,%6,%7}, [%8+16];"
                  : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
                  : "l"(p));
 }
@@ -237,8 +238,7 @@ __device__ __forceinline__ float gather_blend_mma(const nsb_field_params &P, flo
 // Quad-cooperative index computation (warp-specialised kernel).
 // In gather_issue every lane of a quad (q = 0..3, the four 32 B pieces of one 128 B line) repeats the same
 // position -> corner -> hash/stride -> trilinear-weight arithmetic for its corner g: 4x redundant, ~80 instructions per
-// level and lane, and the gather warps are issue-limited (ncu r1: 64 % issue-active, 1 instruction per 11 cycles and
-// warp).  Here the 32 lanes compute 32 DISTINCT (level, corner) pairs -- lane L: level 4U + (L >> 3), corner L & 7 --
+// level and lane, and the gather warps are issue-limited.  Here the 32 lanes compute 32 DISTINCT (level, corner) pairs -- lane L: level 4U + (L >> 3), corner L & 7 --
 // once per four levels, and each tile's issue fetches the two (entry, weight) pairs it needs with shuffles.
 // Same per-pair arithmetic in the same order as gather_issue: bit-identical results.
 // -------------------------------------------------------------------------------------------
@@ -291,12 +291,11 @@ __device__ __forceinline__ void gather_issue_q(const nsb_field_params &P, const 
 // and Q its quad 0; on return they hold the NEXT sample's (when next_xs != nullptr; next_out = that sample's smem row).
 // The 8 lanes (q == 0) that own a level quad's features store them to the shared-memory feature row as soon as the
 // quad is reduced (no yv[4] carried to a final 4-shuffle delivery), and the next sample's position is read from
-// shared memory when its first loads are issued (not held across the body): the gather role runs in 64 registers,
-// and a spill inside this loop is very expensive (L1 is flooded by the streaming table lines: 48 spill instructions
-// per sample took the kernel from 2.6 to 4.0 ms).
-// (Tried and dropped, r1e: feeding the HMMA A fragment straight from the LDG.256 registers -- m16 row halves = even /
-// odd members of ONE line, B in 4 registers, no IMAD.MOV -- 790 instead of 980 instructions per sample but 2.56 vs
-// 2.20 ms: the extra shuffle per level sits on the per-warp dependent chain, and the loop is latency-, not issue-bound.)
+// shared memory when its first loads are issued (not held across the body): register pressure in the gather role is
+// what decides its speed, and a spill inside this loop is very expensive (L1 is flooded by the streaming table lines).
+// (Tried and dropped: feeding the HMMA A fragment straight from the load registers -- m16 row halves = even / odd
+// members of ONE line -- takes fewer instructions per sample but puts an extra shuffle per level on the per-warp
+// dependent chain, and the loop is latency-, not issue-bound.)
 // B fragments parked in a lane-private shared-memory column ([k-step][lane] uint2 = {b0, b1}) and fetched one k-step
 // at a time: rebuilt only when the timestep changes, and 8 registers that are not live across the sample loop.
 struct BlendBSmem {
@@ -327,7 +326,7 @@ __device__ __forceinline__ float gather_consume(const GatherTile &G, const Blend
 }
 
 // L2 prefetch of a quad's 32 lines (hashed levels only: the dense levels mostly hit L1/L2 anyway).  Costs no registers
-// beyond the address; issued one quad ahead so that the LDG.256 that land in registers find their line in L2.
+// beyond the address; issued one quad ahead so that the loads that land in registers find their line in L2.
 __device__ __forceinline__ void quad_prefetch(const nsb_field_params &P, const uint8_t *tab_base, const QuadIdx &Q, int U, int lane) {
     if (P.levels.hashed[4 * U + (lane >> 3)])
         asm volatile("prefetch.global.L2 [%0];" ::"l"(tab_base + (size_t)Q.entry * 128));

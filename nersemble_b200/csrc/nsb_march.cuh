@@ -116,7 +116,7 @@ __device__ __forceinline__ int32_t march_occ_ray(const nsb_march_args &a, const 
         const int ovf[3] = {fin[0] + stp[0], fin[1] + stp[1], fin[2] + stp[2]};
         // The DDA's cell sequence does not depend on the occupancy bits, so it runs kAhead cells ahead of the sample
         // emission: the kAhead occupancy loads of a group are independent (one L2 round trip per group instead of one
-        // per cell -- with 4096 rays = 4096 threads the marcher is pure latency: 0.46 -> see profiles/README.md).
+        // per cell -- with 4096 rays = 4096 threads the marcher is pure latency).
         // Cells are processed in the original order with the original arithmetic: bit-identical samples.
         constexpr int kAhead = 4;
         bool finished = false;

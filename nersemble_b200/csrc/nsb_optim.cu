@@ -31,9 +31,8 @@ __global__ void __launch_bounds__(kOptWarps * 32) table_step_kernel(const __grid
     for (int sl = 0; sl < kOptMaxSlots; ++sl) cw[sl] = sl < n_slots ? a.cw_slots[sl * NSB_MEMBERS + lane] : 0.f;
     const int64_t E = a.total_entries;
     const int64_t n_blocks = (E + kOptLines - 1) / kOptLines;
-    const float w1 = 1.0f - a.beta1, w2 = 1.0f - a.beta2;
-    const float step_size = a.lr / a.bias_correction1;
-    const float bc2_sqrt = sqrtf(a.bias_correction2);
+    const float w1 = a.one_minus_beta1, w2 = a.one_minus_beta2;
+    const float step_size = a.step_size, bc2_sqrt = a.bias_correction2_sqrt;
     for (int64_t blk = (int64_t)blockIdx.x * kOptWarps + warp; blk < n_blocks; blk += (int64_t)gridDim.x * kOptWarps) {
         const int64_t e0 = blk * kOptLines;
         if (ADAM) {   // pull the NEXT block's p / m / v lines (3 x 8 KB) into L2 while this one is processed
@@ -66,7 +65,7 @@ __global__ void __launch_bounds__(kOptWarps * 32) table_step_kernel(const __grid
         }
         __syncwarp();
         const int lines = (int)min((int64_t)kOptLines, E - e0);
-        constexpr int U = 4;    // lines in flight per warp: 12 x 256 B loads outstanding (one line at a time: 2.9 TB/s)
+        constexpr int U = 4;    // lines in flight per warp: 12 x 256 B loads outstanding (one line at a time leaves HBM idle)
         for (int j0 = 0; j0 < lines; j0 += U) {
             float2 p[U], m[U], v[U], d[U];
 #pragma unroll
@@ -107,12 +106,16 @@ __global__ void __launch_bounds__(kOptWarps * 32) table_step_kernel(const __grid
                 }
                 float2 pp = p[u], mm = m[u], vv = v[u];
                 if (a.weight_decay != 0.f) { g0 = fmaf(a.weight_decay, pp.x, g0); g1 = fmaf(a.weight_decay, pp.y, g1); }
-                // torch.optim.Adam (_single_tensor_adam): exp_avg.lerp_(grad, 1 - beta1); exp_avg_sq.mul_(beta2).addcmul_(g, g, 1 - beta2);
-                // denom = exp_avg_sq.sqrt() / sqrt(bias_correction2) + eps; param.addcdiv_(exp_avg, denom, -lr / bias_correction1)
+                // torch.optim.Adam on CUDA (_multi_tensor_adam), operation by operation and with its roundings, so that
+                // the step is bit-identical to torch's for the same gradient:
+                //   exp_avg.lerp_(grad, 1 - beta1)                 m + w1 * (g - m), one fma
+                //   exp_avg_sq.mul_(beta2).addcmul_(g, g, 1 - beta2)   v * beta2 rounded, then v + w2 * (g * g), one fma
+                //   denom = exp_avg_sq.sqrt() / sqrt(bc2) + eps;  param.addcdiv_(exp_avg, denom, -lr / bc1)   one fma
                 mm.x = fmaf(w1, g0 - mm.x, mm.x); mm.y = fmaf(w1, g1 - mm.y, mm.y);
-                vv.x = fmaf(w2 * g0, g0, vv.x * a.beta2); vv.y = fmaf(w2 * g1, g1, vv.y * a.beta2);
-                pp.x -= step_size * (mm.x / (sqrtf(vv.x) / bc2_sqrt + a.eps));
-                pp.y -= step_size * (mm.y / (sqrtf(vv.y) / bc2_sqrt + a.eps));
+                vv.x = fmaf(w2, __fmul_rn(g0, g0), __fmul_rn(vv.x, a.beta2));
+                vv.y = fmaf(w2, __fmul_rn(g1, g1), __fmul_rn(vv.y, a.beta2));
+                pp.x = fmaf(-step_size, __fdiv_rn(mm.x, __fadd_rn(__fdiv_rn(__fsqrt_rn(vv.x), bc2_sqrt), a.eps)), pp.x);
+                pp.y = fmaf(-step_size, __fdiv_rn(mm.y, __fadd_rn(__fdiv_rn(__fsqrt_rn(vv.y), bc2_sqrt), a.eps)), pp.y);
                 *reinterpret_cast<float2 *>(a.tables + o) = pp;
                 *reinterpret_cast<float2 *>(a.exp_avg + o) = mm;
                 *reinterpret_cast<float2 *>(a.exp_avg_sq + o) = vv;
@@ -128,8 +131,8 @@ static int opt_grid() {
     int dev = 0, sms = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 148;
-    return sms * 8;   // 32 KB of shared memory per block: 7 blocks fit, 8 x 148 keeps every SM at its residency limit
+    if (sms <= 0) sms = 132;
+    return sms * 8;   // 32 KB of shared memory per block: 7 blocks fit, 8 per SM keeps every SM at its residency limit
 }
 
 }  // namespace nsb
@@ -144,7 +147,10 @@ extern "C" int nsb_table_adam_step(const nsb_table_adam_args *args, void *stream
         set_error("nsb_table_adam_step: rank-1 workspace needs cw_slots and 1 <= n_slots <= 32");
         return 1;
     }
-    if (!(args->bias_correction1 > 0.f) || !(args->bias_correction2 > 0.f)) { set_error("nsb_table_adam_step: bias corrections must be > 0 (step >= 1)"); return 1; }
+    if (!(args->bias_correction1 > 0.f) || !(args->bias_correction2 > 0.f) || !(args->bias_correction2_sqrt > 0.f)) {
+        set_error("nsb_table_adam_step: bias corrections must be > 0 (step >= 1)");
+        return 1;
+    }
     AdamK K;
     K.a = *args;
     table_step_kernel<true><<<opt_grid(), kOptWarps * 32, 0, (cudaStream_t)stream>>>(K, nullptr);

@@ -1,4 +1,4 @@
-// Ray marching, visibility filter and alpha compositing for sm_100a.
+// Ray marching, visibility filter and alpha compositing for sm_90a.
 //
 // Replaces (reference, relative to /root/reference/src/nersemble/nerfstudio/):
 //   nerfacc OccGridEstimator.sampling -> traverse_grids   (model_components/nersemble_volumetric_sampler.py:95-108)

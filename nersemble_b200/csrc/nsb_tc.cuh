@@ -1,5 +1,5 @@
-// tcgen05 / TMEM primitives for the 5th-generation tensor cores of sm_100a (inline PTX; descriptor bit layouts as in
-// CUTLASS cute/arch/mma_sm100_desc.hpp: UMMA::SmemDescriptor / UMMA::InstrDescriptor).
+// Warpgroup MMA (wgmma) primitives for the Hopper tensor cores of sm_90a (inline PTX; descriptor bit layout as in
+// CUTLASS cute/arch/mma_sm90_desc.hpp: GMMA::GmmaDescriptor).
 #pragma once
 #include "nsb_common.cuh"
 
@@ -9,99 +9,58 @@ namespace tc {
 // Shared-memory matrix descriptor, K-major, no swizzle ("interleave"): the operand is tiled in 8 x 16-byte core
 // matrices (8 rows of 8 halfs, 128 contiguous bytes); LBO = byte distance between the two core matrices of one K = 16
 // step, SBO = byte distance between consecutive 8-row groups.  Bits: [0,14) address >> 4, [16,30) LBO >> 4,
-// [32,46) SBO >> 4, [46,48) version = 1 (Blackwell), [61,64) layout type = 0 (SWIZZLE_NONE).
+// [32,46) SBO >> 4, [49,52) base offset = 0, [62,64) layout type = 0 (INTERLEAVE).
 __device__ __forceinline__ uint64_t smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     return (uint64_t)((smem_addr >> 4) & 0x3fffu) | ((uint64_t)((lbo_bytes >> 4) & 0x3fffu) << 16) |
-           ((uint64_t)((sbo_bytes >> 4) & 0x3fffu) << 32) | (1ull << 46);
-}
-// Instruction descriptor for kind::f16: D = F32 (bits [4,6) = 1), A = B = F16 (0), both K-major, N >> 3 at [17,23),
-// M >> 4 at [24,29).
-__host__ __device__ constexpr uint32_t instr_desc_f16(int M, int N) {
-    return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+           ((uint64_t)((sbo_bytes >> 4) & 0x3fffu) << 32);
 }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t *dst_smem, uint32_t ncols) {     // one full warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {       // the allocating warp
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 // generic-proxy shared-memory writes -> visible to the async proxy (the tensor core reads operands through it)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// orders this thread's earlier register / shared-memory accesses before the wgmma operations that follow
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// D[tmem] (+)= A[smem] . B[smem]^T, M x N x 16, issued by ONE thread
-__device__ __forceinline__ void mma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, bool accumulate) {
+// D[64 x 64] (+)= A[64 x 16] . B[64 x 16]^T, both operands K-major in shared memory, fp16 in, fp32 accumulate; issued by
+// the whole warpgroup.  D fragment: thread t = 32 w + l holds rows 16 w + l / 4 (+ 8) and columns 8 j + 2 (l % 4) (+ 1)
+// in d[4 j + 2 * (row half) + (column parity)].
+__device__ __forceinline__ void mma_m64n64k16(float (&d)[32], uint64_t a_desc, uint64_t b_desc, bool accumulate) {
     asm volatile(
         "{\n\t"
         ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"((uint32_t)accumulate)
-        : "memory");
-}
-// the mbarrier receives one arrival when every MMA issued so far by this thread has completed
-__device__ __forceinline__ void commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// TMEM -> registers: lane = 32 * (warp % 4) + laneid, N consecutive fp32 columns
-__device__ __forceinline__ void ld32(uint32_t taddr, float (&v)[32]) {
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
         "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-          "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-          "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "%32, %33, p, 1, 1, 0, 0;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a_desc), "l"(b_desc), "r"((uint32_t)accumulate)
         : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
 }
-// 16 columns, NO wait: pair with wait_ld() (tcgen05.wait::ld waits for every outstanding load of the thread, so a
-// software pipeline is  wait -> issue next -> process current)
-__device__ __forceinline__ void ld16_nowait(uint32_t taddr, uint32_t (&r)[16]) {
+// D[64 x 16] (+)= A[64 x 16] . B[16 x 16]^T, same fragment layout (j < 2)
+__device__ __forceinline__ void mma_m64n16k16(float (&d)[8], uint64_t a_desc, uint64_t b_desc, bool accumulate) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(a_desc), "l"(b_desc), "r"((uint32_t)accumulate)
         : "memory");
-}
-__device__ __forceinline__ void ld8_nowait(uint32_t taddr, uint32_t (&r)[8]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                 : "r"(taddr)
-                 : "memory");
-}
-__device__ __forceinline__ void wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void ld8(uint32_t taddr, float (&v)[8]) {
-    uint32_t r[8];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                 : "r"(taddr)
-                 : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
 }
 
-// exactly one lane of a converged warp (the issuing lane of tcgen05.mma / commit / bulk copies)
+// exactly one lane of a converged warp (the issuing lane of the bulk copies)
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;
     asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
     return pred != 0;
-}
-// (x0, x1) += (b0, b1) as ONE packed fp32x2 add (sm_100: FADD2)
-__device__ __forceinline__ void add_f32x2(float &x0, float &x1, float b0, float b1) {
-    asm("{\n\t.reg .b64 a, b, d;\n\tmov.b64 a, {%0, %1};\n\tmov.b64 b, {%2, %3};\n\tadd.rn.f32x2 d, a, b;\n\tmov.b64 {%0, %1}, d;\n\t}"
-        : "+f"(x0), "+f"(x1)
-        : "f"(b0), "f"(b1));
 }
 // half2(relu(lo), relu(hi)), round-to-nearest: the ReLU rides on the conversion
 __device__ __forceinline__ uint32_t cvt_relu_h2(float lo, float hi) {

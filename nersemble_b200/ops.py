@@ -1,7 +1,7 @@
 """Tensor-level wrappers over the libnsb C ABI (include/nsb.h).
 
 PyTorch is used for device memory and streams only; all arithmetic of the hot path runs in
-the hand-written sm_100a kernels.  There is no CPU fallback: non-CUDA tensors raise.
+the hand-written sm_90a kernels.  There is no CPU fallback: non-CUDA tensors raise.
 """
 from __future__ import annotations
 
@@ -16,7 +16,8 @@ from . import _lib, packing
 
 _F32 = torch.float32
 
-# Deformation MLP of the inference kernels on tcgen05 / TMEM (NativeParams.build(tcgen05=...) overrides it per instance;
+# Deformation MLP of the inference kernels on wgmma (the "tcgen05" flag keeps its original name; NativeParams.build(tcgen05=...)
+# overrides it per instance;
 # NSB_TCGEN05=0/1 in the environment overrides the default).
 import os as _os
 USE_TCGEN05 = _os.environ.get("NSB_TCGEN05", "1") == "1"
@@ -53,7 +54,7 @@ def _rows(n: int, tail=(), dtype=_F32, device=None, zero: bool = False) -> torch
     """[n, *tail] as a view of an allocation rounded up to 65 536 rows.  The packed sample count changes every training
     step (stratified jitter); exact-size allocations of the large per-sample buffers (2.7 GB of saved activations at
     1.8 M samples) then miss the caching allocator's free blocks whenever the count grows and fall through to
-    cudaMalloc -- measured: 11 ms of host time per forward, 47 ms per step with the backward buffers (r2 profile)."""
+    cudaMalloc, which costs host time on every forward and more with the backward buffers."""
     n_alloc = max(((int(n) + _ROW_QUANTUM - 1) // _ROW_QUANTUM) * _ROW_QUANTUM, 1)
     t = (torch.zeros if zero else torch.empty)((n_alloc,) + tuple(tail), dtype=dtype, device=device)
     return t[:n]
@@ -85,7 +86,7 @@ class NativeParams:
     deform_packed_tb: Optional[torch.Tensor] = None   # half, fragment order, no warp-code columns
     deform_code_w: Optional[list] = None              # (stem_w[0], stem_w[4], stem_b[0], stem_b[4]): per-sample code bias
     deform_code_bias: Optional[torch.Tensor] = None   # float [T, 2, 128]
-    deform_packed_umma: Optional[torch.Tensor] = None # half, tcgen05 core-matrix order (inference kernels; opt-in)
+    deform_packed_umma: Optional[torch.Tensor] = None # half, wgmma core-matrix order (inference kernels; opt-in)
 
     def __post_init__(self):
         self.aabb_list = [float(v) for v in self.aabb.detach().cpu().reshape(-1)]
@@ -138,7 +139,7 @@ class NativeParams:
     def frame_table(self, uniform_time: float, window_hash, disable_initial: bool, soft_transition: bool) -> Optional[torch.Tensor]:
         """float [total_entries, 2]: the tables blended with the member weights of ONE timestep (nsb_blend_tables), for
         calls whose samples all carry `uniform_time` (a camera frame).  Cached per (timestep, window, table version); None
-        when the tcgen05 inference kernels (the only ones that read it) are not in use."""
+        when the wgmma inference kernels (the only ones that read it) are not in use."""
         if getattr(self, "_umma_src", None) is None or self.tables is None or self.blend_codes is None:
             return None
         import numpy as np
@@ -158,11 +159,11 @@ class NativeParams:
 
     def c_params(self, inference: bool = False, frame: Optional[torch.Tensor] = None) -> _lib.FieldParams:
         """inference: the call saves nothing for a backward pass -- the kernels may then run the deformation MLP on
-        tcgen05 / TMEM, which takes its weights in another order (packed here on first use: a training step never pays)."""
+        wgmma, which takes its weights in another order (packed here on first use: a training step never pays)."""
         if inference and self.deform_packed_umma is None and getattr(self, "_umma_src", None) is not None:
             self.deform_packed_umma = packing.pack_deform_umma_fast(*self._umma_src)
         p = getattr(self, "_cp", None)      # the level table / aabb part never changes: fill it once (host time matters:
-        fresh = p is None                   # a training step is ~6 ms of host work against ~20 ms of GPU work)
+        fresh = p is None                   # a training step has little GPU time to hide host work behind)
         if fresh:
             p = self._cp = _lib.FieldParams()
         p.tables = _ptr(self.tables)
@@ -428,8 +429,11 @@ def table_adam_step(tables: torch.Tensor, exp_avg: torch.Tensor, exp_avg_sq: tor
         a.g_rank1, a.cw_slots, a.n_slots = _ptr(pending["g_rank1"]), _ptr(pending["cw_slots"]), int(pending["n_slots"])
     a.grad_scale = float(grad_scale)
     a.lr, a.beta1, a.beta2, a.eps, a.weight_decay = float(lr), float(betas[0]), float(betas[1]), float(eps), float(weight_decay)
-    a.bias_correction1 = 1.0 - float(betas[0]) ** step
-    a.bias_correction2 = 1.0 - float(betas[1]) ** step
+    bc1, bc2 = 1.0 - float(betas[0]) ** step, 1.0 - float(betas[1]) ** step
+    a.bias_correction1, a.bias_correction2 = bc1, bc2
+    # the scalars exactly as torch.optim.Adam (_multi_tensor_adam) forms them: Python doubles, rounded once to float
+    a.step_size, a.bias_correction2_sqrt = float(lr) / bc1, bc2 ** 0.5
+    a.one_minus_beta1, a.one_minus_beta2 = 1.0 - float(betas[0]), 1.0 - float(betas[1])
     _lib.check(lib.nsb_table_adam_step(C.byref(a), _stream()), "nsb_table_adam_step")
 
 

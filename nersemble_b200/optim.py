@@ -2,8 +2,8 @@
 
 The reference trains with nerfstudio's AdamOptimizerConfig (torch.optim.Adam, eps = 1e-15) over the 8 dense tcnn grid
 gradients (train_nersemble.py: optimizers["fields"]).  For the 403 M-element table that costs, per step, the dense
-expansion of the scattered gradient (3.1 ms), torch's multi-pass foreach Adam (6.0 ms) and a fresh fp32 -> fp16 copy
-of the table for the next forward (r1d profile, 1 x B200).  `FusedFieldsAdam` is a torch.optim.Adam whose update of
+expansion of the scattered gradient, torch's multi-pass foreach Adam and a fresh fp32 -> fp16 copy
+of the table for the next forward.  `FusedFieldsAdam` is a torch.optim.Adam whose update of
 the table parameter is nsb_table_adam_step: rank-1 gradient expansion + Adam + fp16 refresh in one streaming pass;
 every other parameter of the group goes through torch.optim.Adam unchanged, and the optimiser state keeps torch's
 keys (`step`, `exp_avg`, `exp_avg_sq`), so checkpoints interchange with a plain Adam.

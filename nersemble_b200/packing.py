@@ -1,4 +1,4 @@
-"""Host-side parameter layout for the B200 kernels (pure torch ops; runs on CPU or GPU).
+"""Host-side parameter layout for the CUDA kernels (pure torch ops; runs on CPU or GPU).
 
 * hash tables: 8 tcnn grids (flat [(entry)*8 + p*2 + f], the reference's
   `field.hash_ensemble.hash_encodings.{c}.params`) <-> native [entry][member=c*4+p][feat] fp16,
@@ -177,7 +177,7 @@ def pack_field_bwd(base_w: Sequence[torch.Tensor], head_w: Sequence[torch.Tensor
 
 # ------------------------------------------------------------------ gather plans
 # Training re-packs the MLP weights every step (they change every step).  The packers above are the definition of the
-# layouts but cost ~300 small torch ops per step (advanced indexing per layer: r1d profile, 9 ms of CPU time, more than
+# layouts but cost ~300 small torch ops per step (advanced indexing per layer: host time comparable to
 # the GPU time of the forward).  A plan is the same packer traced once on int64 element ids: afterwards packing is
 # cat(sources) -> one gather -> half.
 _PLANS: dict = {}
@@ -251,7 +251,7 @@ def pack_all_fast(stem_w, r_w, v_w, base_w, head_w):
 
 
 def _umma_block(Wb: torch.Tensor) -> torch.Tensor:
-    """[N, 64] (N % 8 == 0) -> the tcgen05 K-major no-swizzle core-matrix order: 8 x 8 fp16 core matrices (8 rows x 16 B),
+    """[N, 64] (N % 8 == 0) -> the wgmma K-major no-swizzle core-matrix order: 8 x 8 fp16 core matrices (8 rows x 16 B),
     byte offset = (n / 8) * 1024 + (k / 8) * 128 + (n % 8) * 16 + (k % 8) * 2  (descriptor LBO = 128, SBO = 1024)."""
     N = Wb.shape[0]
     assert Wb.shape[1] == 64 and N % 8 == 0
@@ -265,7 +265,7 @@ def _pad2(W: torch.Tensor, rows: int, cols: int) -> torch.Tensor:
 
 
 def pack_deform_umma(stem_w, r_w, v_w) -> torch.Tensor:
-    """Deformation weights for the tcgen05 tensor role (nsb_field_tensor_role_tc.inc): 14 blocks in order of use, each
+    """Deformation weights for the wgmma tensor role (nsb_field_tensor_role_tc.inc): 14 blocks in order of use, each
     [n x 64 k] in core-matrix order (_umma_block).  K follows the reference's input column order
     (windowed_nerf_encoding.py:50-73: sin 21 | cos 21 | 2 pi p 3), zero-padded to 64; the 128 warp-code columns of
     layers 0 and 4 are not here (they enter as the per-timestep code bias, deform_code_bias):

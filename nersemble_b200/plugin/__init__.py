@@ -2,7 +2,7 @@
 
 Same class names, constructor/forward signatures, config dataclasses, output keys and
 state_dict keys as /root/reference/src/nersemble/nerfstudio/** (cited per class), with all
-arithmetic behind libnsb (CUDA, sm_100a).  NeRSembleNGPModel.get_outputs is differentiable
+arithmetic behind libnsb (CUDA, sm_90a).  NeRSembleNGPModel.get_outputs is differentiable
 (fused forward + backward kernels); the stand-alone component modules are forward-only and
 raise when called with autograd enabled instead of silently returning graph-less tensors.
 """

@@ -97,7 +97,7 @@ class HashEnsemble(nn.Module):
     Storage.  The reference holds 8 tcnn grids of 8 features/level (`hash_encodings.{c}.params`, flat fp32).  Here the
     ONE trainable tensor is `tables`, fp32 [total_entries, 32 members, 2 feats] -- the layout the kernels gather (one
     128-byte fp16 line per entry) and scatter gradients into, so a training step never permutes 1.6 GB between
-    layouts (r1d profile: ~13 ms of index/cat/copy glue per step).  state_dict()/load_state_dict() still speak the
+    layouts (index/cat/copy glue every step).  state_dict()/load_state_dict() still speak the
     reference's keys and flat shapes (hooks below), and the parameter sits in the same `fields` group.  The fp16 copy
     the forward kernels read is a cache refreshed when `tables` changes (or written by the fused optimiser)."""
 
@@ -106,7 +106,7 @@ class HashEnsemble(nn.Module):
         hc = config.hash_encoding_config
         assert config.n_hash_encodings == 32 and hc.n_features_per_level == 2 and hc.n_levels == 16 \
             and hc.n_dims_to_encode == 3 and hc.interpolation == 'Linear', \
-            "the B200 kernels are specialised for the reference configuration: 32 x (16 levels, 2 features), Linear"
+            "the CUDA kernels are specialised for the reference configuration: 32 x (16 levels, 2 features), Linear"
         self.n_hash_encodings = config.n_hash_encodings
         self.hash_encoding_config = hc
         self.disable_initial_hash_ensemble = config.disable_initial_hash_ensemble
@@ -234,7 +234,7 @@ class SE3WarpingField(nn.Module):
         super().__init__()
         assert config.n_freq_pos == 7 and config.warp_code_dim == 128 and config.mlp_num_layers == 6 and \
             config.mlp_layer_width == 128 and tuple(config.skip_connections) == (4,), \
-            "the B200 kernels are specialised for the reference deformation field (7 freqs, 128-d code, 6x128, skip 4)"
+            "the CUDA kernels are specialised for the reference deformation field (7 freqs, 128-d code, 6x128, skip 4)"
         in_dim = 3 * 7 * 2 + 3 + config.warp_code_dim
         w = config.mlp_layer_width
         self.mlp_stem = _MLP([(w, in_dim), (w, w), (w, w), (w, w), (w, w + in_dim), (w, w)])

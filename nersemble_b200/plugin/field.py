@@ -44,7 +44,7 @@ class NeRSembleNeRFactoField(nn.Module):
         bad = [k for k, v in unsupported.items() if v]
         if bad or spatial_distortion is not None or spherical_harmonics_degree != 0 or not use_hash_ensemble:
             raise NotImplementedError(
-                f"B200 field supports the NeRSemble recipe only (train_nersemble.py:184-240): hash ensemble, "
+                f"the CUDA field supports the NeRSemble recipe only (train_nersemble.py:184-240): hash ensemble, "
                 f"identity direction encoding, no scene contraction; got {bad}, sh_degree={spherical_harmonics_degree}")
         assert num_layers == 2 and hidden_dim == 64 and geo_feat_dim == 15 and num_layers_color == 3 and hidden_dim_color == 64
         self.register_buffer("aabb", aabb)

@@ -197,7 +197,7 @@ class NeRSembleNGPModel(Model):
         self.use_fused_sampler = True    # training: march / density pre-pass / visibility / packing with one host sync
         self.frame_tables = True         # eval frames (one timestep per camera frame): gather a per-frame blended table
         self.frame_table_min_rays = 16384  # ... for frames of at least this many rays (the check is one host sync per frame,
-                                           # the table one 0.17 ms pass over the hash tables)
+                                           # the table one streaming pass over the hash tables)
         self.prepass_reuse = True        # ... and the pre-pass's blended features / corner values are packed with the kept
                                          # samples, so the differentiable forward does not gather the tables a second time
 
@@ -587,7 +587,7 @@ class NeRSembleNGPModel(Model):
 
     def _loss_dict_sync_free(self, outputs, batch) -> Dict[str, Tensor]:
         """Same six losses (models/base.py:90-249) without device->host synchronisation: the reference selects
-        elements with boolean indexing and `if mask.any()` (11 `nonzero` syncs per step in the r1e profile, each draining
+        elements with boolean indexing and `if mask.any()` (11 `nonzero` syncs per step, each draining
         the launch queue).  Here every masked mean is sum(mask * x) / count on the device.  Differences a caller can
         see: a term whose mask is empty is PRESENT with value 0 (the reference omits the key); values agree to
         summation order."""

@@ -8,14 +8,14 @@ restatements, [3P-mem], parity unpinned); the glue restated here is pinned by
 tests/golden/*.npz, which oracle/gen_golden.py produced by running the REAL reference
 modules (imported from /root/reference) on the same inputs.
 
-Parameters are held in the B200-native layout (FieldParams): one hash table
+Parameters are held in the kernels' native layout (FieldParams): one hash table
 [entry][member(32)][feat(2)] instead of 8 tcnn grids of 8 features; `tables_from_tcnn` /
 `tables_to_tcnn` convert (hash_ensemble.py:112 rearrange 'b c (l p f) -> b (l f) (c p)').
 
 Precision modes (oracle.tp.tcnn_cpu.Precision.mode):
   "reference": fp16 roundings where the reference has them (tcnn half interpolation and
                outputs, fp16 window product / einsum output, autocast fp16 Linear outputs)
-  "kernel":    roundings of the B200 kernels (fp16-stored tables/weights, fp16 MLP inputs and
+  "kernel":    roundings of the CUDA kernels (fp16-stored tables/weights, fp16 MLP inputs and
                hidden activations, fp32 everywhere else)
   "none":      fp16-stored tables/weights only
 """

@@ -16,7 +16,7 @@ model_components/nersemble_volumetric_sampler.py:95-108;
 model_components/nersemble_deformation_renderer.py:22-25.
 
 The marcher is a per-ray Python loop in numpy float32 scalars with the operation order
-of the CUDA kernel (no fused multiply-add) so the B200 marcher can be bit-exact to it.
+of the CUDA kernel (no fused multiply-add) so the CUDA marcher can be bit-exact to it.
 PARITY UNPINNED for this layer (no nerfacc source / golden vectors available).
 
 Upstream map (nerfacc v0.5.2, KAIR-BAIR/nerfacc):

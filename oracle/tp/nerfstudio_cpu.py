@@ -153,7 +153,7 @@ class MLP(nn.Module):
         """nn.Linear under the active precision emulation: "reference"+autocast = fp16 operands
         and fp16 output (torch.autocast in engine/nersemble_trainer.py:182; eval and the
         occupancy callback run WITHOUT autocast -> fp32); "kernel" = fp16 operands, fp32
-        accumulate and bias (the B200 kernel)."""
+        accumulate and bias (the CUDA kernel)."""
         from .tcnn_cpu import Precision, half_round
         if Precision.mode == "kernel":
             return half_round(x) @ half_round(layer.weight).t() + layer.bias

@@ -54,7 +54,7 @@ class Precision:
 
     mode "reference": every rounding tcnn applies (half interpolation fma, half output,
                       half MLP activations) -- closest to what the reference executes.
-    mode "kernel":    the roundings of the B200 kernels: fp16-stored tables and weights,
+    mode "kernel":    the roundings of the CUDA kernels: fp16-stored tables and weights,
                       fp32 interpolation/blend, activations rounded to fp16 between
                       MLP layers, fp32 accumulation.
     mode "none":      fp16-stored tables/weights only; all math fp32.

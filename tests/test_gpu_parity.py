@@ -45,7 +45,7 @@ def trained_mma(trained):
 @pytest.mark.parametrize("tensor_role", ["tcgen05", "mma.sync"])
 @pytest.mark.parametrize("w_hash,w_deform", [(32.0, 7.0), (1.5, 3.3), (1, 0.0), (None, None)])
 def test_field_and_composite_vs_oracle(trained, trained_mma, w_hash, w_deform, tensor_role):
-    """Both inference instantiations of the deformation MLP against the oracle: the tcgen05 / TMEM role (the default,
+    """Both inference instantiations of the deformation MLP against the oracle: the wgmma role (flag name "tcgen05", the default,
     nsb_field_tensor_role_tc.inc) and the mma.sync role (NSB_TCGEN05=0; also what the training kernels run)."""
     from nersemble_b200 import ops
     P, NP = trained if tensor_role == "tcgen05" else trained_mma

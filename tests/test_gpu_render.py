@@ -121,7 +121,7 @@ def test_occupancy_scan_over_many_rays_and_capacity_overflow(trained):
 def test_plugin_eval_paths_use_the_fused_render(trained, monkeypatch, tensor_role):
     """NeRSembleNGPModel eval: get_outputs_for_camera_ray_bundle (no host sync) and get_outputs (full contract) agree bit
     for bit with the training-path kernels run in eval mode when both run the mma.sync deformation role; with the
-    tcgen05 role (the default of the fused render) they agree to fp16-operand rounding."""
+    wgmma role (flag name "tcgen05", the default of the fused render) they agree to fp16-operand rounding."""
     from nersemble_b200 import ops
     from nersemble_b200.nerfstudio_shim import RayBundle
     monkeypatch.setattr(ops, "USE_TCGEN05", tensor_role == "tcgen05")

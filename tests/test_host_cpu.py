@@ -158,7 +158,7 @@ def test_gather_plans_reproduce_the_packers():
 
 
 def test_pack_deform_umma_layout():
-    """tcgen05 B operands (packing.pack_deform_umma): 14 blocks per tile in order of use, [n x 64 k] in K-major
+    """wgmma B operands (packing.pack_deform_umma): 14 blocks per tile in order of use, [n x 64 k] in K-major
     no-swizzle core-matrix order -- byte offset (n/8)*1024 + (k/8)*128 + (n%8)*16 + (k%8)*2 (descriptor LBO 128, SBO 1024);
     K = the reference's encoding column order, zero padded; the gather-plan version is identical."""
     from nersemble_b200 import packing as pk
@@ -181,8 +181,8 @@ def test_pack_deform_umma_layout():
 
 
 def test_forward_kernel_gather_role_has_no_spill_storm():
-    """Regression guard for a performance cliff, not for correctness: local-memory traffic inside the 64-register gather
-    role of field_kernel_ws is catastrophic (48 spill instructions per sample: 2.6 -> 4.0 ms on B200, profiles/README.md)
+    """Regression guard for a performance cliff, not for correctness: local-memory traffic inside the gather
+    role of field_kernel_ws is catastrophic (a spill inside the sample loop costs more than the loop's own work)
     and ptxas allocates that role erratically.  The committed source builds with <= 9 STL/LDL there; fail loudly when a
     change (or a different toolkit) pushes a variant over 16."""
     import shutil, subprocess
@@ -196,8 +196,8 @@ def test_forward_kernel_gather_role_has_no_spill_storm():
     assert len(rows) >= 12
     for r in rows:
         assert int(r[r.index("gather") + 1]) <= 16, out
-    # the tcgen05 instantiations (the default for inference): the committed source builds with 4-6 (per-sample blend) and
-    # 0-6 (frame table) spill instructions in the gather role
+    # the wgmma instantiations (the default for inference): the committed source builds with at most 2 spill instructions
+    # in the gather role
     out = subprocess.run([sys.executable, os.path.join(ROOT, "tools", "spill_report.py"), obj, "kernel_tc"], capture_output=True, text=True).stdout
     rows = [l.split() for l in out.splitlines() if "gather" in l]
     assert len(rows) >= 8
@@ -264,10 +264,10 @@ def test_rank1_slot_map_for_many_timesteps():
 
 
 def test_posenc_sine_reduction_constants():
-    """tc::sin_reduced (nsb_tc.cuh) = two-constant Cody-Waite reduction to [-pi, pi] + MUFU.SIN, the posenc of the tcgen05
+    """tc::sin_reduced (nsb_tc.cuh) = two-constant Cody-Waite reduction to [-pi, pi] + MUFU.SIN, the posenc of the wgmma
     deformation role.  Emulated in numpy (fp32 operands, the FMA's exact product in float64): over the argument range of
     the encoding -- fl(2 pi p) * 2^j for j < 7 and positions up to 4 box widths outside the box -- the REDUCTION moves the
-    sine by < 2e-7 (MUFU.SIN adds < 4e-7 on the reduced range, B300_MICROARCH); the value then becomes an fp16 MMA operand
+    sine by < 2e-7 (MUFU.SIN adds < 4e-7 on the reduced range); the value then becomes an fp16 MMA operand
     (spacing 4.9e-4 near 1), as in the oracle's kernel mode."""
     import numpy as np
     rng = np.random.default_rng(0)

@@ -79,7 +79,7 @@ def test_losses():
 
 
 def test_precision_modes_within_rgb_tolerance():
-    """The fp16 roundings of the reference ("reference") and of the B200 kernels ("kernel") both stay
+    """The fp16 roundings of the reference ("reference") and of the CUDA kernels ("kernel") both stay
     within the north-star tolerance (RGB L2 <= 1e-3) of the fp32 evaluation ("none")."""
     ref, _ = load_golden("fixed_trained_reference")
     ker, _ = load_golden("fixed_trained_kernel")
@@ -92,7 +92,7 @@ def test_precision_modes_within_rgb_tolerance():
 def test_gradients_match_reference_glue_autograd():
     """Backward parity pin: torch autograd through the oracle restatement vs autograd through the UNMODIFIED reference glue
     (golden `grads_train`: one full training step, all six losses, deformation field + hash ensemble) -- every parameter
-    gradient, the table gradient on a seeded 400 k-element sample plus its global / per-level norms."""
+    gradient, the table gradient on a seeded 200 k-element sample plus its global / per-level norms."""
     from oracle.tp.tcnn_cpu import hashgrid_levels
     g, meta = load_golden("grads_train")
     Precision.mode = "none"; Precision.autocast = False
@@ -131,7 +131,7 @@ def test_gradients_match_reference_glue_autograd():
     close(P.r_w.grad, g["r_w_grad"], "r_w", DEF); close(P.r_b.grad, g["r_b_grad"], "r_b", DEF)
     close(P.v_w.grad, g["v_w_grad"], "v_w", DEF); close(P.v_b.grad, g["v_b_grad"], "v_b", DEF)
     flat = P.tables.grad.reshape(-1)
-    pick = torch.randint(0, flat.numel(), (400_000,), generator=torch.Generator().manual_seed(5))
+    pick = torch.randint(0, flat.numel(), (200_000,), generator=torch.Generator().manual_seed(5))
     close(flat[pick], g["tables_grad_sample"], "tables (sample)", 5e-3)
     assert int((flat != 0).sum()) == int(g["tables_grad_nonzeros"])
     sums = torch.stack([flat.double().sum(), (flat.double() ** 2).sum(), flat.double().abs().sum()])

@@ -374,7 +374,7 @@ def test_training_step_gradients_vs_reference_glue_golden():
     check(m.field.mlp_head.params.grad, g["mlp_head_grad"], "mlp_head", 0.12)
     check(m.time_embedding.weight.grad, g["time_emb_grad"], "time_emb", 0.12)
     # deformation branch: the golden is fp32 ('none' precision) while the kernels keep warp codes, activations and
-    # deltas in fp16; measured on B200 for the smallest of these gradients (warp codes, |g| ~ 2e-5): rel 0.09, cos 0.993
+    # deltas in fp16; for the smallest of these gradients (warp codes, |g| ~ 2e-5): rel 0.09, cos 0.993
     check(m.time_embedding_deformation.weight.grad, g["time_emb_deform_grad"], "time_emb_deform", 0.3, 0.97)
     se3 = m.deformation_field.se3_field
     for i, layer in enumerate(se3.mlp_stem.layers):
@@ -383,7 +383,7 @@ def test_training_step_gradients_vs_reference_glue_golden():
     check(se3.mlp_r.layers[0].weight.grad, g["r_w_grad"], "r_w", 0.3, 0.97)
     check(se3.mlp_v.layers[0].weight.grad, g["v_w_grad"], "v_w", 0.3, 0.97)
     flat = m.field.hash_ensemble.tables.grad.reshape(-1).cpu()
-    pick = torch.randint(0, flat.numel(), (400_000,), generator=torch.Generator().manual_seed(5))
+    pick = torch.randint(0, flat.numel(), (200_000,), generator=torch.Generator().manual_seed(5))
     cos = torch.nn.functional.cosine_similarity(flat[pick].reshape(1, -1).double(), g["tables_grad_sample"].reshape(1, -1).double()).item()
     assert cos > 0.99, cos
     assert abs((flat.double() ** 2).sum().item() / g["tables_grad_sums"][1].item() - 1.0) < 0.25

@@ -1,6 +1,6 @@
 """bench.py --config 3 | 4 | 5: the BASELINE.json configurations beyond the headline forward (configs[2..4]).
 
-  3  train_nersemble.py seq-30 default hparams, 1 x B200: one optimiser step = jittered occupancy march + visibility
+  3  train_nersemble.py seq-30 default hparams, 1 x H100: one optimiser step = jittered occupancy march + visibility
      pre-pass (alpha_thre 1e-2) -> differentiable fused render -> six losses -> backward -> FusedFieldsAdam (fields) +
      Adam (embeddings, deformation field).  Synthetic multi-view batch (image, alpha map, depth map per ray).
   4  novel-view frames (default 1088 x 1920, T = 24), rays of every frame sharded 1/N per GPU, per-ray RGB all-gathered
@@ -183,7 +183,7 @@ def run_config4(args):
     assert H % world == 0, "frames are sharded by rows"
     rows = H // world
     # rows are dealt out round-robin (row r -> rank r % N), not in contiguous blocks: the head sits in the middle of the
-    # frame, and with contiguous blocks the central ranks marched 4x the samples of the outer ones (r2m: 8 GPUs only 2.85x)
+    # frame, and with contiguous blocks the central ranks marched 4x the samples of the outer ones
     from nersemble_b200.distributed import gather_rows_round_robin, shard_rows_round_robin
     my_rows = shard_rows_round_robin(H, rank, world, device=dev)
 
@@ -222,7 +222,7 @@ def run_config4(args):
         sampler = B.ClockSampler(D.local_rank)
         if rank == 0:
             sampler.start(); time.sleep(0.05)
-        K = n_frames if args.steps == 20 else args.steps      # default: all 24 timesteps once
+        K = args.steps      # frames rendered; frame f shows timestep f % 24
         ms = B.timed(D, render_frame, K, sampler)
         sampler.stop_flag = True
         # sharded vs unsharded: the last frame again on rank 0 alone (chunk boundaries differ, pixels must not)

@@ -1,5 +1,5 @@
 """Time the stages of the fused field kernel separately (CUDA events) to see where the time goes.
-    python tools/kernel_sweep.py            (on a GPU box)"""
+    python tools/kernel_sweep.py            (on an H100)"""
 import os, sys, json
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -1,5 +1,5 @@
-// Microbenchmark: attainable random-line gather bandwidth on B200 (what bounds the hash gather?).
-//   nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o randgather randgather.cu && ./randgather
+// Microbenchmark: attainable random-line gather bandwidth on H100 (what bounds the hash gather?).
+//   nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o randgather randgather.cu && ./randgather
 // Each thread issues ILP independent 16-byte loads per iteration; 8 consecutive lanes cover one
 // 128-byte line (LINE=128) or 4 lanes cover 64 bytes (LINE=64), line index = hash(counter).
 #include <cstdio>
@@ -31,7 +31,7 @@ __global__ void gather_kernel(const uint4 *__restrict__ tab, uint32_t n_lines, i
 
 template <int ILP, int LPL>
 void run(const uint4 *tab, uint32_t n_lines, uint4 *out, int blocks_per_sm, int threads, const char *name) {
-    int sms = 148; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+    int sms = 132; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
     int blocks = sms * blocks_per_sm;
     int iters = 200;
     cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);

@@ -1,5 +1,5 @@
-"""A/B of the tcgen05 deformation role (field_kernel_tc) against the mma.sync role (field_kernel_ws) on the same samples:
-max |diff| of sigma / rgb / offsets and the kernel time of both.  Run under `timeout` on the GPU box."""
+"""A/B of the wgmma deformation role (flag name "tcgen05") (field_kernel_tc) against the mma.sync role (field_kernel_ws) on the same samples:
+max |diff| of sigma / rgb / offsets and the kernel time of both.  Run under `timeout` on an H100."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch, bench

@@ -1,4 +1,4 @@
-"""Cycle breakdown of the tcgen05 deformation stage (debug build: tools/build_variant.sh tc_prof "-DNSB_TC_PROF",
+"""Cycle breakdown of the wgmma deformation stage (debug build: tools/build_variant.sh tc_prof "-DNSB_TC_PROF",
 run with NSB_LIB=tools/_variants/tc_prof.so): phases of one D-group thread of CTA 3, per tile."""
 import os, sys, ctypes as C
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -13,7 +13,7 @@ tu = torch.full_like(t, 0.5)
 lib = _lib.load()
 lib.nsb_debug_tc_prof.argtypes = [C.c_void_p]
 names = ["outside D (buffer wait, loop)", "input loads", "posenc", "barriers", "MMA (issue+exec+commit) wait", "epilogues", "heads+SE3+xs", "-"]
-tiles = (ts.numel() // 128 + 147 - 3) // 148
+tiles = (ts.numel() // 128 + 131 - 3) // 132
 for label, kw in (("per-sample blend", dict(ray_times=t)), ("frame table", dict(ray_times=tu, uniform_time=0.5)),
                   ("fused render kernel, fixed march, per-sample blend", None)):
     for _ in range(3):
