@@ -71,10 +71,15 @@ typedef struct nsb_field_params {
                                        [128 outputs x 64 inputs] fp16 (heads [16 x 64]) in K-major 8 x 16-byte core matrices
                                        (python: pack_deform_umma; nsb_deform_packed_umma_bytes()).  When set, the inference
                                        kernels run the deformation MLP on wgmma.mma_async (sm_90a warpgroup MMA). */
-    const void *frame_table;   /* optional, float2 [total_entries]: the tables blended with ONE timestep's member weights
-                                  (nsb_blend_tables).  Only valid when EVERY sample of the call has that timestep (one
-                                  camera frame): the gather then reads 8 B per corner from a 50 MB table that stays in L2
-                                  instead of a 128 B line from HBM.  Used by the wgmma inference kernels. */
+    const void *frame_table;   /* optional, float2 [n][total_entries]: the tables blended with the member weights of one or
+                                  more timesteps (nsb_blend_tables).  The gather then reads 8 B per corner instead of a
+                                  128 B line.  Used by the wgmma inference kernels.  With frame_stride == 0 it is ONE
+                                  timestep's table and only valid when EVERY sample of the call has that timestep (one
+                                  camera frame: a 50 MB table that stays in L2). */
+    int64_t frame_stride;      /* entries between consecutive timesteps' tables in frame_table: a sample of timestep t
+                                  gathers from frame_table + t * frame_stride.  total_entries for a stack of all
+                                  n_timesteps tables (rays of mixed timesteps); 0 for one frame table.
+                                  frame_stride * n_timesteps must be < 2^32. */
     const void *field_packed;  /* fp16 mlp_base + mlp_head weights in MMA-B fragment order */
     const void *warp_codes;    /* __half [n_timesteps][128]  (time_embedding_deformation) */
     const float *blend_codes;  /* float  [n_timesteps][32]   (time_embedding) */
@@ -143,11 +148,13 @@ const char *nsb_last_error(void);
 /* Sizes (bytes) of the packed weight buffers the python packer must produce. */
 size_t nsb_deform_packed_bytes(void);
 size_t nsb_deform_packed_umma_bytes(void);
-/* Frame table of one timestep: out[e] = sum_m (blend_codes[timestep][m] * cw_scale[m] + cw_bias[m]) * tables[e][m][:]
- * (float2 per entry, fp32 accumulation) -- HashEnsemble.forward's member blend (hash_ensemble.py:119-139) hoisted out of
- * the per-sample path for calls whose samples all share that timestep (nsb_field_params.frame_table). */
-int nsb_blend_tables(const nsb_field_params *params, const nsb_field_opts *opts, int32_t timestep, int64_t n_entries,
-                     void *out, void *stream);
+/* Frame tables of n_timesteps consecutive timesteps first_timestep, first_timestep + 1, ...:
+ *   out[i][e] = sum_m (blend_codes[first_timestep + i][m] * cw_scale[m] + cw_bias[m]) * tables[e][m][:]
+ * (float2 [n_timesteps][n_entries], fp32 accumulation) -- HashEnsemble.forward's member blend (hash_ensemble.py:119-139)
+ * hoisted out of the per-sample path (nsb_field_params.frame_table / frame_stride).  One pass: every 128 B line is read
+ * once for all n_timesteps outputs, and slice i is bit-identical to the n_timesteps = 1 call for that timestep. */
+int nsb_blend_tables(const nsb_field_params *params, const nsb_field_opts *opts, int32_t first_timestep,
+                     int32_t n_timesteps, int64_t n_entries, void *out, void *stream);
 size_t nsb_field_packed_bytes(void);
 
 /* Fused per-sample field evaluation (deformation MLP -> SE(3) warp -> 32-member hash ensemble

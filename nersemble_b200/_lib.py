@@ -27,7 +27,7 @@ class Levels(C.Structure):
 class FieldParams(C.Structure):
     _fields_ = [("tables", C.c_void_p), ("deform_bias", C.c_void_p),
                 ("deform_packed_tb", C.c_void_p), ("deform_code_bias", C.c_void_p), ("deform_packed_umma", C.c_void_p), ("frame_table", C.c_void_p),
-                ("field_packed", C.c_void_p), ("warp_codes", C.c_void_p), ("blend_codes", C.c_void_p),
+                ("frame_stride", C.c_int64), ("field_packed", C.c_void_p), ("warp_codes", C.c_void_p), ("blend_codes", C.c_void_p),
                 ("n_timesteps", C.c_int32), ("aabb", C.c_float * 6), ("levels", Levels)]
 
 
@@ -151,7 +151,7 @@ SYMBOLS = {
     "nsb_deform_packed_bytes": (C.c_size_t, []),
     "nsb_field_packed_bytes": (C.c_size_t, []),
     "nsb_deform_packed_umma_bytes": (C.c_size_t, []),
-    "nsb_blend_tables": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p]),
+    "nsb_blend_tables": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p]),
     "nsb_field_forward": (C.c_int, [C.POINTER(FieldParams), C.POINTER(FieldOpts), C.POINTER(Samples),
                                     C.POINTER(FieldOut), C.c_void_p]),
     "nsb_field_backward": (C.c_int, [C.POINTER(FieldParams), C.POINTER(FieldOpts), C.POINTER(Samples),

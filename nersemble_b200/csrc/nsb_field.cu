@@ -415,8 +415,10 @@ static_assert(sizeof(SmemTC) <= 227 * 1024, "shared memory plan");
         __syncthreads();                                                                                            \
     }
 
-// FRAME: the gather role reads the member-blended frame table (nsb_field_gather_role_frame.inc)
-template <bool HEAD, bool FRAME>
+// FRAME: the gather role reads the member-blended frame table (nsb_field_gather_role_frame.inc); STACK: one table per
+// timestep (frame_stride != 0).  STACK is a template flag so that the single-frame kernels compile exactly as without the
+// timestep offset: ptxas' allocation of the whole kernel (tensor role included) moves with any change to the gather code.
+template <bool HEAD, bool FRAME, bool STACK>
 __global__ void __launch_bounds__(kLaunchBoundWS, 1) field_kernel_tc(const __grid_constant__ FieldArgs A) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     SmemTC &sm = *reinterpret_cast<SmemTC *>(smem_raw);
@@ -696,7 +698,7 @@ __global__ void __launch_bounds__(kLaunchBoundWS, 1) render_kernel_ws(const __gr
 }
 
 // render_kernel_ws with the deformation MLP on wgmma (nsb_field_tensor_role_tc.inc); SAMPLER 2 or 4
-template <int SAMPLER, bool FRAME>
+template <int SAMPLER, bool FRAME, bool STACK>
 __global__ void __launch_bounds__(kLaunchBoundWS, 1) render_kernel_tc(const __grid_constant__ RenderKArgs K) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     SmemTC &sm = *reinterpret_cast<SmemTC *>(smem_raw);
@@ -823,23 +825,24 @@ static int launch_field_ws(const FieldArgs &A, cudaStream_t st) {
     return save ? launch_field_ws_<D, F, H, true>(A, st) : launch_field_ws_<D, F, H, false>(A, st);
 }
 
-template <bool H, bool FR>
+template <bool H, bool FR, bool ST>
 static int launch_field_tc_(const FieldArgs &A, cudaStream_t st) {
     const size_t smem = sizeof(SmemTC);
     static bool configured = false;
     if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(field_kernel_tc<H, FR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaError_t e = cudaFuncSetAttribute(field_kernel_tc<H, FR, ST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(field_kernel_tc): %s", cudaGetErrorString(e)); return 1; }
         configured = true;
     }
     const int64_t n_tiles = (A.S.n_samples + NSB_TILE - 1) / NSB_TILE;
     const int grid = (int)std::min<int64_t>(n_tiles, (int64_t)num_sms());
-    field_kernel_tc<H, FR><<<grid, kThreadsWS, smem, st>>>(A);
+    field_kernel_tc<H, FR, ST><<<grid, kThreadsWS, smem, st>>>(A);
     return check_launch("field_kernel_tc");
 }
 template <bool H>
 static int launch_field_tc(const FieldArgs &A, cudaStream_t st) {
-    return A.P.frame_table ? launch_field_tc_<H, true>(A, st) : launch_field_tc_<H, false>(A, st);
+    if (!A.P.frame_table) return launch_field_tc_<H, false, false>(A, st);
+    return A.P.frame_stride ? launch_field_tc_<H, true, true>(A, st) : launch_field_tc_<H, true, false>(A, st);
 }
 
 template <bool D>
@@ -855,6 +858,11 @@ static int launch_field_given(const FieldArgs &A, cudaStream_t st) {
     const int grid = (int)std::min<int64_t>(n_tiles, (int64_t)num_sms());
     field_kernel_ws_given<D><<<grid, kThreadsWS, smem, st>>>(A);
     return check_launch("field_kernel_ws_given");
+}
+
+// The frame-table gather forms timestep * frame_stride + entry in 32 bits
+static bool frame_stride_ok(const nsb_field_params *p) {
+    return p->frame_stride >= 0 && p->frame_stride * (int64_t)p->n_timesteps <= (int64_t)UINT32_MAX;
 }
 
 template <bool D, bool F, bool H>
@@ -917,6 +925,7 @@ extern "C" int nsb_field_forward(const nsb_field_params *params, const nsb_field
         return 1;
     }
     if (params->n_timesteps < 1) { set_error("nsb_field_forward: n_timesteps < 1"); return 1; }
+    if (!frame_stride_ok(params)) { set_error("nsb_field_forward: frame_stride out of range"); return 1; }
     FieldArgs A;
     A.P = *params; A.O = *opts; A.S = *samples; A.out = *out;
     for (int k = 0; k < 3; ++k) A.aabb_size[k] = params->aabb[3 + k] - params->aabb[k];
@@ -942,46 +951,60 @@ extern "C" int nsb_hash_blend_forward(const nsb_field_params *params, const nsb_
 }
 
 // -------------------------------------------------------------------------------------------
-// nsb_blend_tables: frame table = the 32 members of every table entry blended with ONE timestep's weights
-// (cw[m] = code[m] * cw_scale[m] + cw_bias[m], hash_ensemble.py:119-139), float2 per entry.  8 lanes per entry
-// (16 B = 4 members each), fp32 accumulation; one streaming pass over the tables (HBM-bound).
+// nsb_blend_tables: frame tables = the 32 members of every table entry blended with the weights of n_ts consecutive
+// timesteps (cw[t][m] = code[t][m] * cw_scale[m] + cw_bias[m], hash_ensemble.py:119-139), float2 per entry and timestep.
+// 8 lanes per entry (16 B = 4 members each), fp32 accumulation, the same member order and xor tree for every timestep;
+// one streaming pass over the tables (each 128 B line read once for all timesteps; the weights sit in shared memory).
 // -------------------------------------------------------------------------------------------
 namespace nsb {
+constexpr int kBlendMaxTimesteps = 256;        // 32 KB of weights in shared memory
 __global__ void __launch_bounds__(256) blend_tables_kernel(const uint4 *__restrict__ tables, const float *__restrict__ code,
                                                            const __grid_constant__ nsb_field_opts O, float2 *__restrict__ out,
-                                                           int64_t n_entries) {
+                                                           int n_ts, int64_t n_entries) {
+    __shared__ float4 cw_s[kBlendMaxTimesteps][8];
     const int lane = threadIdx.x & 31, sub = lane & 7;
-    float cw[4];
+    for (int i = threadIdx.x; i < n_ts * 8; i += blockDim.x) {
+        const int t = i >> 3, s = i & 7;
+        float cw[4];
 #pragma unroll
-    for (int i = 0; i < 4; ++i) cw[i] = fmaf(__ldg(code + 4 * sub + i), O.cw_scale[4 * sub + i], O.cw_bias[4 * sub + i]);
+        for (int k = 0; k < 4; ++k) cw[k] = fmaf(__ldg(code + t * NSB_MEMBERS + 4 * s + k), O.cw_scale[4 * s + k], O.cw_bias[4 * s + k]);
+        cw_s[t][s] = make_float4(cw[0], cw[1], cw[2], cw[3]);
+    }
+    __syncthreads();
     const int64_t stride = (int64_t)gridDim.x * (blockDim.x >> 3);
     for (int64_t e = (int64_t)blockIdx.x * (blockDim.x >> 3) + (threadIdx.x >> 3); e < ((n_entries + 3) & ~(int64_t)3); e += stride) {
-        float f0 = 0.f, f1 = 0.f;
+        float2 f[4] = {};
         if (e < n_entries) {
             const uint4 v = __ldcs(tables + e * 8 + sub);          // streamed once: evict-first
-            const uint32_t u[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const float2 f = unpack_h2(u[i]);
-                f0 = fmaf(cw[i], f.x, f0); f1 = fmaf(cw[i], f.y, f1);
-            }
+            f[0] = unpack_h2(v.x); f[1] = unpack_h2(v.y); f[2] = unpack_h2(v.z); f[3] = unpack_h2(v.w);
         }
+        for (int t = 0; t < n_ts; ++t) {
+            const float4 c4 = cw_s[t][sub];
+            const float cw[4] = {c4.x, c4.y, c4.z, c4.w};
+            float f0 = 0.f, f1 = 0.f;
 #pragma unroll
-        for (int o = 1; o < 8; o <<= 1) { f0 += __shfl_xor_sync(0xffffffffu, f0, o); f1 += __shfl_xor_sync(0xffffffffu, f1, o); }
-        if (sub == 0 && e < n_entries) out[e] = make_float2(f0, f1);
+            for (int i = 0; i < 4; ++i) { f0 = fmaf(cw[i], f[i].x, f0); f1 = fmaf(cw[i], f[i].y, f1); }
+#pragma unroll
+            for (int o = 1; o < 8; o <<= 1) { f0 += __shfl_xor_sync(0xffffffffu, f0, o); f1 += __shfl_xor_sync(0xffffffffu, f1, o); }
+            if (sub == 0 && e < n_entries) out[(int64_t)t * n_entries + e] = make_float2(f0, f1);
+        }
     }
 }
 }  // namespace nsb
 
-extern "C" int nsb_blend_tables(const nsb_field_params *params, const nsb_field_opts *opts, int32_t timestep, int64_t n_entries,
-                                void *out, void *stream) {
+extern "C" int nsb_blend_tables(const nsb_field_params *params, const nsb_field_opts *opts, int32_t first_timestep,
+                                int32_t n_timesteps, int64_t n_entries, void *out, void *stream) {
     if (!params || !opts || !out || !params->tables || !params->blend_codes) { set_error("nsb_blend_tables: null argument"); return 1; }
-    if (timestep < 0 || timestep >= params->n_timesteps) { set_error("nsb_blend_tables: timestep out of range"); return 1; }
+    if (first_timestep < 0 || n_timesteps < 1 || n_timesteps > kBlendMaxTimesteps || first_timestep > params->n_timesteps - n_timesteps) {
+        set_error("nsb_blend_tables: timesteps [%d, %d + %d) out of range (n_timesteps %d, at most %d per call)", first_timestep,
+                  first_timestep, n_timesteps, params->n_timesteps, kBlendMaxTimesteps);
+        return 1;
+    }
     if (n_entries <= 0) return 0;
     const int blocks = (int)std::min<int64_t>((n_entries + 31) / 32, (int64_t)num_sms() * 8);
     blend_tables_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const uint4 *>(params->tables),
-                                                                  params->blend_codes + (size_t)timestep * NSB_MEMBERS, *opts,
-                                                                  reinterpret_cast<float2 *>(out), n_entries);
+                                                                  params->blend_codes + (size_t)first_timestep * NSB_MEMBERS, *opts,
+                                                                  reinterpret_cast<float2 *>(out), n_timesteps, n_entries);
     return check_launch("blend_tables_kernel");
 }
 
@@ -992,12 +1015,12 @@ namespace nsb {
 constexpr size_t kRenderHdrBytes = 64, kRenderPartials = 1024;
 static_assert(sizeof(nsb_render_ws_header) == kRenderHdrBytes, "workspace header layout");
 
-template <int SAMPLER, bool FR>
+template <int SAMPLER, bool FR, bool ST>
 static int launch_render_tc_(const RenderKArgs &K, cudaStream_t st) {
     const size_t smem = sizeof(SmemTC);
     static bool configured = false;
     if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(render_kernel_tc<SAMPLER, FR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaError_t e = cudaFuncSetAttribute(render_kernel_tc<SAMPLER, FR, ST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(render_kernel_tc): %s", cudaGetErrorString(e)); return 1; }
         configured = true;
     }
@@ -1006,13 +1029,14 @@ static int launch_render_tc_(const RenderKArgs &K, cudaStream_t st) {
     cudaError_t e = cudaMemsetAsync(&K.hdr->barrier, 0, sizeof(uint32_t), st);
     if (e != cudaSuccess) { set_error("nsb_render_forward: memset: %s", cudaGetErrorString(e)); return 2; }
     void *kargs[] = {const_cast<RenderKArgs *>(&K)};
-    e = cudaLaunchCooperativeKernel(reinterpret_cast<const void *>(render_kernel_tc<SAMPLER, FR>), dim3(grid), dim3(kThreadsWS), kargs, smem, st);
+    e = cudaLaunchCooperativeKernel(reinterpret_cast<const void *>(render_kernel_tc<SAMPLER, FR, ST>), dim3(grid), dim3(kThreadsWS), kargs, smem, st);
     if (e != cudaSuccess) { set_error("render_kernel_tc: %s", cudaGetErrorString(e)); return 2; }
     return check_launch("render_kernel_tc");
 }
 template <int SAMPLER>
 static int launch_render_tc(const RenderKArgs &K, cudaStream_t st) {
-    return K.F.P.frame_table ? launch_render_tc_<SAMPLER, true>(K, st) : launch_render_tc_<SAMPLER, false>(K, st);
+    if (!K.F.P.frame_table) return launch_render_tc_<SAMPLER, false, false>(K, st);
+    return K.F.P.frame_stride ? launch_render_tc_<SAMPLER, true, true>(K, st) : launch_render_tc_<SAMPLER, true, false>(K, st);
 }
 
 template <bool D, int SAMPLER>
@@ -1060,6 +1084,7 @@ extern "C" int nsb_render_forward(const nsb_field_params *params, const nsb_fiel
         return 1;
     }
     if (params->n_timesteps < 1 || ra->capacity <= 0) { set_error("nsb_render_forward: n_timesteps < 1 or capacity <= 0"); return 1; }
+    if (!frame_stride_ok(params)) { set_error("nsb_render_forward: frame_stride out of range"); return 1; }
     if (ra->sampler == 0) {
         if (ra->n_per_ray <= 0 || ra->capacity < ra->n_rays * (int64_t)ra->n_per_ray) { set_error("nsb_render_forward: capacity < n_rays * n_per_ray"); return 1; }
     } else if (ra->sampler == 1 || ra->sampler == 3) {

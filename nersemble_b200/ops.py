@@ -152,14 +152,36 @@ class NativeParams:
             out = cached[1] if cached is not None else torch.empty((self.tables.shape[0], 2), dtype=_F32, device=self.tables.device)
             opts = make_opts(window_hash, None, True, True, disable_initial, soft_transition)
             cp = self.c_params()
-            _lib.check(_lib.load().nsb_blend_tables(C.byref(cp), C.byref(opts), tsi, int(self.tables.shape[0]), _ptr(out), _stream()),
+            _lib.check(_lib.load().nsb_blend_tables(C.byref(cp), C.byref(opts), tsi, 1, int(self.tables.shape[0]), _ptr(out), _stream()),
                        "nsb_blend_tables")
             self._frame = cached = (key, out)
         return cached[1]
 
+    def timestep_tables(self, window_hash, disable_initial: bool, soft_transition: bool) -> Optional[torch.Tensor]:
+        """float [T, total_entries, 2]: frame_table of every timestep, stacked (one nsb_blend_tables pass), for calls whose
+        samples carry mixed timesteps: the gather then reads one 8 B entry per corner instead of a 128 B line.  Cached
+        per (window, table version).  None when the wgmma inference kernels are not in use, or when the stack would be
+        more than twice the size of the line tables (T > 32): the line gather is then the cheaper path."""
+        if getattr(self, "_umma_src", None) is None or self.tables is None or self.blend_codes is None:
+            return None
+        T, E = self.n_timesteps, int(self.tables.shape[0])
+        if T * E * 8 > 2 * self.tables.nbytes or T * E > 0xFFFFFFFF:      # the kernels index the stack in 32 bits
+            return None
+        key = (None if window_hash is None else float(window_hash), bool(disable_initial), bool(soft_transition),
+               self.tables.data_ptr(), self.tables._version, self.blend_codes.data_ptr(), self.blend_codes._version)
+        cached = getattr(self, "_stack", None)
+        if cached is None or cached[0] != key:
+            out = cached[1] if cached is not None else torch.empty((T, E, 2), dtype=_F32, device=self.tables.device)
+            opts = make_opts(window_hash, None, True, True, disable_initial, soft_transition)
+            cp = self.c_params()
+            _lib.check(_lib.load().nsb_blend_tables(C.byref(cp), C.byref(opts), 0, T, E, _ptr(out), _stream()), "nsb_blend_tables")
+            self._stack = cached = (key, out)
+        return cached[1]
+
     def c_params(self, inference: bool = False, frame: Optional[torch.Tensor] = None) -> _lib.FieldParams:
         """inference: the call saves nothing for a backward pass -- the kernels may then run the deformation MLP on
-        wgmma, which takes its weights in another order (packed here on first use: a training step never pays)."""
+        wgmma, which takes its weights in another order (packed here on first use: a training step never pays).
+        frame: a frame_table [E, 2] (every sample has its timestep) or a timestep_tables stack [T, E, 2]."""
         if inference and self.deform_packed_umma is None and getattr(self, "_umma_src", None) is not None:
             self.deform_packed_umma = packing.pack_deform_umma_fast(*self._umma_src)
         p = getattr(self, "_cp", None)      # the level table / aabb part never changes: fill it once (host time matters:
@@ -172,6 +194,7 @@ class NativeParams:
         p.deform_code_bias = _ptr(self.deform_code_bias)
         p.deform_packed_umma = _ptr(self.deform_packed_umma) if inference else None
         p.frame_table = _ptr(frame) if (inference and self.deform_packed_umma is not None) else None
+        p.frame_stride = int(frame.shape[1]) if (p.frame_table and frame.dim() == 3) else 0
         p.field_packed = _ptr(self.field_packed)
         p.warp_codes = _ptr(self.warp_codes)
         p.blend_codes = _ptr(self.blend_codes)
@@ -218,8 +241,10 @@ def field_forward(P: NativeParams, *, window_hash=None, window_deform=None, use_
                   sample_warp_codes=None, n_samples_dev: Optional[torch.Tensor] = None,
                   given_feat: Optional[torch.Tensor] = None, uniform_time: Optional[float] = None,
                   want: Sequence[str] = ("sigma", "rgb", "offsets"),
-                  disable_initial: bool = True, soft_transition: bool = True) -> Dict[str, torch.Tensor]:
-    """Fused deformation + hash ensemble + field MLPs for packed samples (nsb_field_forward)."""
+                  disable_initial: bool = True, soft_transition: bool = True, line_gather: bool = False) -> Dict[str, torch.Tensor]:
+    """Fused deformation + hash ensemble + field MLPs for packed samples (nsb_field_forward).
+    Inference calls gather member-blended tables (NativeParams.frame_table for a uniform_time, timestep_tables
+    otherwise) when the wgmma kernels run; line_gather=True forces the per-sample blend of the 128 B table lines."""
     lib = _lib.load()
     ray_based = origins is not None
     keep = []
@@ -295,9 +320,12 @@ def field_forward(P: NativeParams, *, window_hash=None, window_deform=None, use_
     inference = (use_deformation and n_samples_dev is None and given_feat is None and sample_warp_codes is None
                  and not any(k in want for k in ("feat", "xs", "corner_vals", "deform_acts")))
     frame = None
-    if inference and uniform_time is not None and sample_blend_codes is None and ("sigma" in want or "rgb" in want):
-        # every sample carries this time (the caller's promise, e.g. one camera frame): gather the blended frame table
-        frame = P.frame_table(uniform_time, window_hash, disable_initial, soft_transition)
+    if inference and not line_gather and sample_blend_codes is None and ("sigma" in want or "rgb" in want):
+        if uniform_time is not None:
+            # every sample carries this time (the caller's promise, e.g. one camera frame): gather the blended frame table
+            frame = P.frame_table(uniform_time, window_hash, disable_initial, soft_transition)
+        else:
+            frame = P.timestep_tables(window_hash, disable_initial, soft_transition)
     cp = P.c_params(inference=inference, frame=frame)
     rc = lib.nsb_field_forward(C.byref(cp), C.byref(opts), C.byref(s), C.byref(o), _stream())
     _lib.check(rc, "nsb_field_forward")
@@ -794,14 +822,16 @@ def render_rays(P: NativeParams, origins, directions, ray_times, *, window_hash=
                 near_plane: float = 0.0, near_planes=None, far_planes=None, binaries=None, aabbs=None,
                 step: float = 1e-3, cone_angle: float = 0.0, capacity: Optional[int] = None,
                 disable_initial=True, soft_transition=True, single_launch: bool = False,
-                single_traversal: bool = True, uniform_time: Optional[float] = None) -> RenderResult:
+                single_traversal: bool = True, uniform_time: Optional[float] = None, line_gather: bool = False) -> RenderResult:
     """The fused inference render (nsb_render_forward): sampler -> field -> composite without a host synchronisation.
     sampler 'fixed' (n_per_ray steps from the box entry: ONE launch) or 'occupancy' (nerfacc march of `binaries`
     [levels,res,res,res] within per-ray near_planes / far_planes: the cooperative march launch + one fused launch;
     single_launch=True marches inside the fused kernel, levels == 1 only; single_traversal=False: count | scan | fill
     instead of one traversal into per-ray slots + a packing copy).  Returns the per-ray outputs (rgb, accumulation,
     depth, deformation, num_samples_per_ray, packed_info); `.packed()` gives the per-sample arrays (one sync).
-    capacity: per-sample workspace size; default = an upper bound of the march (rays x ceil(largest diagonal / step) + 2)."""
+    capacity: per-sample workspace size; default = an upper bound of the march (rays x ceil(largest diagonal / step) + 2).
+    The field gathers member-blended tables (frame_table for a uniform_time, timestep_tables otherwise) unless
+    line_gather=True forces the per-sample blend of the 128 B table lines."""
     lib = _lib.load()
     origins, directions = _f32c(origins).reshape(-1, 3), _f32c(directions).reshape(-1, 3)
     ray_times = None if ray_times is None else _f32c(ray_times).reshape(-1)
@@ -861,9 +891,12 @@ def render_rays(P: NativeParams, origins, directions, ray_times, *, window_hash=
         return out
     opts = make_opts(window_hash, window_deform, use_deformation, True, disable_initial, soft_transition)
     frame = None
-    if uniform_time is not None and use_deformation and not single_launch:
-        # all rays carry this time (one camera frame): the member blend is hoisted into a per-frame table (frame_table)
-        frame = P.frame_table(uniform_time, window_hash, disable_initial, soft_transition)
+    if use_deformation and not single_launch and not line_gather:
+        if uniform_time is not None:
+            # all rays carry this time (one camera frame): the member blend is hoisted into a per-frame table (frame_table)
+            frame = P.frame_table(uniform_time, window_hash, disable_initial, soft_transition)
+        else:
+            frame = P.timestep_tables(window_hash, disable_initial, soft_transition)
     cp = P.c_params(inference=True, frame=frame)
     _lib.check(lib.nsb_render_forward(C.byref(cp), C.byref(opts), C.byref(a), _stream()), "nsb_render_forward")
     return out

@@ -195,7 +195,8 @@ class NeRSembleNGPModel(Model):
         self.lpips = None                # optional callable(image[1,3,H,W], rgb[1,3,H,W]) -> scalar (needs pretrained weights)
         self.use_fused_render = True     # eval renders: sampler -> field -> composite fused, no host sync (ops.render_rays)
         self.use_fused_sampler = True    # training: march / density pre-pass / visibility / packing with one host sync
-        self.frame_tables = True         # eval frames (one timestep per camera frame): gather a per-frame blended table
+        self.frame_tables = True         # eval renders gather member-blended tables: per frame (one timestep per camera
+                                         # frame) or per timestep (mixed-time bundles); False: per-sample blend of the lines
         self.frame_table_min_rays = 16384  # ... for frames of at least this many rays (the check is one host sync per frame,
                                            # the table one streaming pass over the hash tables)
         self.prepass_reuse = True        # ... and the pre-pass's blended features / corner values are packed with the kept
@@ -339,7 +340,7 @@ class NeRSembleNGPModel(Model):
                                use_deformation=cfg.use_deformation_field, training=self.training, sampler="occupancy",
                                near_planes=near_planes, far_planes=far_planes, binaries=og.binaries, aabbs=og.aabbs,
                                step=cfg.render_step_size, cone_angle=cfg.cone_angle, uniform_time=uniform_time,
-                               **self._blend_opts())
+                               line_gather=not self.frame_tables, **self._blend_opts())
 
     @torch.no_grad()
     def _sample_packed(self, ray_bundle: RayBundle, jitter: Optional[Tensor], want_payload: bool = False):
