@@ -370,10 +370,13 @@ __device__ unsigned long long g_tc_prof[8], g_tc_prof_k[8];
 #else
 #define KPROF(i)
 #endif
-#ifndef NSB_TC_SPLIT
-#define NSB_TC_SPLIT 1      // deformation (wgmma) and density / colour MLPs (mma.sync) on separate warp groups
-#endif
 constexpr size_t kTcPackedBytes = 12 * 16384 + 2 * 2048;
+
+// Warp index that ptxas can see is uniform across the warp (lane 0's value, broadcast).  With `tid >> 5`, ptxas cannot
+// prove that the role split `warp < kTensorWarps` keeps whole warpgroups together, inserts a warpgroup arrive in the
+// divergent path and serialises every wgmma.mma_async of the deformation chain (ptxas C7520).  The *_ws kernels keep
+// `tid >> 5`: there the broadcast moves their gather-role register allocation and adds spills in the sample loop.
+__device__ __forceinline__ int tc_warp_index(int tid) { return __shfl_sync(0xffffffffu, tid >> 5, 0); }
 
 struct alignas(1024) SmemTC {
     uint8_t wring[kTcStages][16384];        // weight blocks [128 n x 64 k] (heads: [16 x 64]) in core-matrix order
@@ -381,8 +384,9 @@ struct alignas(1024) SmemTC {
     uint8_t act[2][32768];                  // hidden activations A operand [128 rows x 128 k], ping-pong between layers
     uint4 field_w[kFieldPackedU4];
     alignas(16) float bias[kBiasFloats];
-    uint64_t full[kTcStages], empty[kTcStages], f_done[2];
+    uint64_t full[kTcStages];
     uint64_t xs_full[2], feat_full[2];
+    uint32_t ring_rel[kTcStages];           // releases of each weight-ring stage by the two tensor warpgroups (2 per use)
     int row_ts[NSB_TILE];                   // timestep of each row of the tile in flight (its code-bias row)
     int tile_ctr[2];
     int64_t n_dyn;
@@ -394,6 +398,7 @@ struct alignas(1024) SmemTC {
     uint4 cv_stage[kGatherWarps][1];        // SAVE is never instantiated with the tc role; the gather include names it
 };
 static_assert(sizeof(SmemTC) <= 227 * 1024, "shared memory plan");
+static_assert(kTensorWarps == 8, "the wgmma tensor role runs two warpgroups of 64 rows");
 
 // setup shared by the tc kernels (textual for the same reason as the other role bodies)
 #define NSB_TC_SETUP()                                                                                              \
@@ -403,10 +408,9 @@ static_assert(sizeof(SmemTC) <= 227 * 1024, "shared memory plan");
         for (int i = tid; i < kBiasFloats; i += kThreadsWS) sm.bias[i] = __ldg(A.P.deform_bias + i);               \
         for (int i = tid; i < (int)(sizeof(sm.a_enc) / 16); i += kThreadsWS) reinterpret_cast<uint4 *>(&sm.a_enc)[i] = make_uint4(0u, 0u, 0u, 0u); \
         if (tid == 0) {                                                                                             \
-            for (int s = 0; s < kTcStages; ++s) { mbar_init(&sm.full[s], 1); mbar_init(&sm.empty[s], 1); }         \
-            mbar_init(&sm.f_done[0], 4); mbar_init(&sm.f_done[1], 4);                                               \
+            for (int s = 0; s < kTcStages; ++s) { mbar_init(&sm.full[s], 1); sm.ring_rel[s] = 0; }                \
             for (int b = 0; b < 2; ++b) {                                                                           \
-                mbar_init(&sm.xs_full[b], 4);                                                                       \
+                mbar_init(&sm.xs_full[b], kTensorWarps);                                                            \
                 mbar_init(&sm.feat_full[b], kGatherWarps);                                                          \
                 sm.tile_ctr[b] = 0;                                                                                 \
             }                                                                                                       \
@@ -422,7 +426,7 @@ template <bool HEAD, bool FRAME, bool STACK>
 __global__ void __launch_bounds__(kLaunchBoundWS, 1) field_kernel_tc(const __grid_constant__ FieldArgs A) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     SmemTC &sm = *reinterpret_cast<SmemTC *>(smem_raw);
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tc_warp_index(tid);
     constexpr bool FIELD = true, SAVE = false, FEAT_GIVEN = false;
 #define NSB_N_SAMPLES A.S.n_samples
     NSB_TC_SETUP()
@@ -703,7 +707,7 @@ __global__ void __launch_bounds__(kLaunchBoundWS, 1) render_kernel_tc(const __gr
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     SmemTC &sm = *reinterpret_cast<SmemTC *>(smem_raw);
     const FieldArgs &A = K.F;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tc_warp_index(tid);
     constexpr bool FIELD = true, HEAD = true, SAVE = false, FEAT_GIVEN = false;
 #define NSB_N_SAMPLES (*reinterpret_cast<const volatile int64_t *>(&sm.n_dyn))
     KPROF(0)

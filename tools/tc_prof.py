@@ -1,5 +1,6 @@
 """Cycle breakdown of the wgmma deformation stage (debug build: tools/build_variant.sh tc_prof "-DNSB_TC_PROF",
-run with NSB_LIB=tools/_variants/tc_prof.so): phases of one D-group thread of CTA 3, per tile."""
+run with NSB_LIB=tools/_variants/tc_prof.so): phases of thread 33 of CTA 3 (warpgroup 0, a row's sine / SE(3) thread),
+per tile: the deformation of its 64 rows, then the density / colour MLPs of its warp's 16 rows."""
 import os, sys, ctypes as C
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch, bench
@@ -12,7 +13,8 @@ ts, te, ri, info = ops.march_fixed(o, d, P.aabb, bench.SAMPLES_PER_RAY, bench.ST
 tu = torch.full_like(t, 0.5)
 lib = _lib.load()
 lib.nsb_debug_tc_prof.argtypes = [C.c_void_p]
-names = ["outside D (buffer wait, loop)", "input loads", "posenc", "barriers", "MMA (issue+exec+commit) wait", "epilogues", "heads+SE3+xs", "-"]
+names = ["feature wait + loop", "input loads", "posenc", "barriers", "MMA (issue+exec+commit) wait", "epilogues", "heads+SE3+xs",
+         "density / colour MLPs"]
 tiles = (ts.numel() // 128 + 131 - 3) // 132
 for label, kw in (("per-sample blend", dict(ray_times=t)), ("frame table", dict(ray_times=tu, uniform_time=0.5)),
                   ("fused render kernel, fixed march, per-sample blend", None)):
