@@ -365,7 +365,8 @@ __global__ void __launch_bounds__(kLaunchBoundWS, 1) field_kernel_ws_given(const
 constexpr int kFrameGatherWarps = NSB_FRAME_GATHER_WARPS;   // frame-table gather: how many of the gather warps do work
 constexpr int kTcStages = 4, kTcBlocksPerTile = 14;
 #ifdef NSB_TC_PROF
-__device__ unsigned long long g_tc_prof[8], g_tc_prof_k[8];
+constexpr int kTcProfPhases = 9;     // tools/tc_prof.py names them
+__device__ unsigned long long g_tc_prof[kTcProfPhases], g_tc_prof_k[8];
 #define KPROF(i) if (threadIdx.x == 0 && blockIdx.x == 3) g_tc_prof_k[i] = (unsigned long long)clock64();
 #else
 #define KPROF(i)
@@ -380,13 +381,13 @@ __device__ __forceinline__ int tc_warp_index(int tid) { return __shfl_sync(0xfff
 
 struct alignas(1024) SmemTC {
     uint8_t wring[kTcStages][16384];        // weight blocks [128 n x 64 k] (heads: [16 x 64]) in core-matrix order
-    uint8_t a_enc[16384];                   // posenc A operand [128 rows x 64 k]
-    uint8_t act[2][32768];                  // hidden activations A operand [128 rows x 128 k], ping-pong between layers
+    uint8_t a_enc[16384];                   // posenc A operand [128 rows x 64 k] (the hidden layers' A stays in registers)
     uint4 field_w[kFieldPackedU4];
     alignas(16) float bias[kBiasFloats];
+    alignas(16) float heads[2][64][8];      // deformation head outputs (v 0..2, r 3..5) of each warpgroup's 64 rows
     uint64_t full[kTcStages];
     uint64_t xs_full[2], feat_full[2];
-    uint32_t ring_rel[kTcStages];           // releases of each weight-ring stage by the two tensor warpgroups (2 per use)
+    uint32_t ring_rel[kTcStages];           // releases of each weight-ring stage by the 8 tensor warps (8 per use)
     int row_ts[NSB_TILE];                   // timestep of each row of the tile in flight (its code-bias row)
     int tile_ctr[2];
     int64_t n_dyn;
@@ -896,8 +897,8 @@ extern "C" size_t nsb_deform_packed_bytes(void) { return (size_t)kTbNumSlabs * k
 extern "C" size_t nsb_field_packed_bytes(void) { return kFieldPackedU4 * sizeof(uint4); }
 extern "C" size_t nsb_deform_packed_umma_bytes(void) { return kTcPackedBytes; }
 #ifdef NSB_TC_PROF
-extern "C" int nsb_debug_tc_prof(unsigned long long *out8) {
-    return (int)cudaMemcpyFromSymbol(out8, nsb::g_tc_prof, sizeof(unsigned long long) * 8);
+extern "C" int nsb_debug_tc_prof(unsigned long long *out) {      // kTcProfPhases cycle counters
+    return (int)cudaMemcpyFromSymbol(out, nsb::g_tc_prof, sizeof(unsigned long long) * kTcProfPhases);
 }
 extern "C" int nsb_debug_tc_prof_kernel(unsigned long long *out8) {      // clock64 at the phase boundaries of render_kernel_tc
     return (int)cudaMemcpyFromSymbol(out8, nsb::g_tc_prof_k, sizeof(unsigned long long) * 8);

@@ -56,6 +56,42 @@ __device__ __forceinline__ void mma_m64n16k16(float (&d)[8], uint64_t a_desc, ui
         : "memory");
 }
 
+// Register-A forms ("RS": A from registers, B from shared memory).  The fp16 A fragment of one k = 16 step is four
+// half2 registers: thread t = 32 w + l holds row 16 w + l / 4 in a[0] (columns 2 (l % 4) + {0, 1}) and a[2] (columns
+// 8 + 2 (l % 4) + {0, 1}), and row 16 w + l / 4 + 8 in a[1] / a[3] (same columns).  That is the D fragment above: the
+// fp32 d[4 j .. 4 j + 3] of 8-column groups j = 2 s and 2 s + 1, converted pairwise to half2, are exactly
+//   a[s] = {h2(d[8 s], d[8 s + 1]), h2(d[8 s + 2], d[8 s + 3]), h2(d[8 s + 4], d[8 s + 5]), h2(d[8 s + 6], d[8 s + 7])},
+// so one layer's output feeds the next layer's A operand with no data movement between threads.  The A registers must
+// be written before the wg_fence that precedes the MMAs reading them (else ptxas serialises the chain, info C7513).
+__device__ __forceinline__ void mma_m64n64k16_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t b_desc, bool accumulate) {
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "{%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"((uint32_t)accumulate)
+        : "memory");
+}
+__device__ __forceinline__ void mma_m64n16k16_rs(float (&d)[8], const uint32_t (&a)[4], uint64_t b_desc, bool accumulate) {
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %13, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, 0;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"((uint32_t)accumulate)
+        : "memory");
+}
+
 // exactly one lane of a converged warp (the issuing lane of the bulk copies)
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;

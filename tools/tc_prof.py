@@ -13,8 +13,8 @@ ts, te, ri, info = ops.march_fixed(o, d, P.aabb, bench.SAMPLES_PER_RAY, bench.ST
 tu = torch.full_like(t, 0.5)
 lib = _lib.load()
 lib.nsb_debug_tc_prof.argtypes = [C.c_void_p]
-names = ["feature wait + loop", "input loads", "posenc", "barriers", "MMA (issue+exec+commit) wait", "epilogues", "heads+SE3+xs",
-         "density / colour MLPs"]
+names = ["feature wait + loop", "input loads", "posenc", "posenc barrier", "MMA (issue+exec+commit) wait",
+         "epilogues, layers 1-3 and 5", "heads+SE3+xs", "density / colour MLPs", "epilogues, layers 0 and 4 (code bias)"]
 tiles = (ts.numel() // 128 + 131 - 3) // 132
 for label, kw in (("per-sample blend", dict(ray_times=t)), ("frame table", dict(ray_times=tu, uniform_time=0.5)),
                   ("fused render kernel, fixed march, per-sample blend", None)):
@@ -26,7 +26,7 @@ for label, kw in (("per-sample blend", dict(ray_times=t)), ("frame table", dict(
             ops.field_forward(P, window_hash=32.0, window_deform=7.0, want=("sigma", "rgb", "offsets"), origins=o, directions=d,
                               t_starts=ts, t_ends=te, ray_indices=ri, **kw)
     torch.cuda.synchronize()
-    buf = (C.c_ulonglong * 8)()
+    buf = (C.c_ulonglong * len(names))()
     assert lib.nsb_debug_tc_prof(buf) == 0
     tot = sum(buf)
     print(f"== {label}: {tiles} tiles on CTA 3, {tot / tiles:.0f} cycles per tile")
