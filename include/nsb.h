@@ -17,6 +17,7 @@
  *                          NeRSembleNeRFactoField.forward (nerfstudio/fields/nersemble_nerfacto_field.py:385-402)
  *                          and NeRSembleNGPModel.field_density_fn (nerfstudio/models/nersemble_instant_ngp.py:235-266)
  *   nsb_hash_blend_forward HashEnsemble.forward alone (component API)
+ *   nsb_hash_blend_backward torch autograd through HashEnsemble.forward alone (component API)
  *   nsb_composite_forward  nerfacc.pack_info / render_weight_from_density + RGB/Depth/Accumulation/
  *                          Deformation renderers (nersemble_instant_ngp.py:325-343,359-362;
  *                          nerfstudio/model_components/nersemble_deformation_renderer.py:10-29)
@@ -24,7 +25,8 @@
  *                          (nerfstudio/model_components/nersemble_volumetric_sampler.py:95-108)
  *   nsb_visibility_*       nerfacc render_visibility_from_density (the training pre-pass of sampling())
  *   nsb_composite_backward / nsb_field_backward / nsb_deform_backward
- *                          torch autograd through all of the above (training)
+ *                          torch autograd through all of the above (training; with per-sample conditioning codes also
+ *                          for the stand-alone field and deformation modules of the component API)
  *   nsb_table_adam_step    torch.optim.Adam on the 8 tcnn grid tensors (scripts/train/train_nersemble.py:243-247) and
  *                          tcnn's per-call fp32 -> fp16 cast of the table parameters
  */
@@ -166,6 +168,13 @@ int nsb_field_forward(const nsb_field_params *params, const nsb_field_opts *opts
  * out_is_half: 1 -> __half output, 0 -> float. */
 int nsb_hash_blend_forward(const nsb_field_params *params, const nsb_field_opts *opts, const float *x,
                            const float *codes, int64_t n, void *out, int32_t out_is_half, void *stream);
+/* Backward of nsb_hash_blend_forward for d_out float [n][32] (output order l*2+f), the same opts as the forward:
+ *   d_tables fp32 [total_entries][32][2], ACCUMULATED (+=), NULL: skip;  d_codes [n][32] and d_x [n][3], written, NULL: skip.
+ * The blend weights are rounded to fp16 like the forward's; a member whose weight the window fixes (w == 1 with
+ * disable_initial_hash_ensemble) gets a code gradient of exactly 0. */
+int nsb_hash_blend_backward(const nsb_field_params *params, const nsb_field_opts *opts, const float *x,
+                            const float *codes, int64_t n, const float *d_out, float *d_tables, float *d_codes,
+                            float *d_x, void *stream);
 
 /* Alpha compositing of packed samples. packed_info int64 [n_rays][2] = (start, count). */
 typedef struct nsb_composite_args {
@@ -208,9 +217,9 @@ typedef struct nsb_field_bwd_args {
     const void *feat;             /* __half [n][32] */
     const float *xs;              /* [n][4] */
     const float *sigma;           /* [n] */
-    const float *rgb;             /* [n][3] */
+    const float *rgb;             /* [n][3] (may be NULL when d_rgb is: density only) */
     const float *d_sigma;         /* [n] */
-    const float *d_rgb;           /* [n][3] */
+    const float *d_rgb;           /* [n][3] or NULL */
     float loss_scale;             /* MLP deltas are fp16 MMA operands: incoming grads are multiplied by this, outputs divided */
     float *d_feat;                /* [n][32] workspace/out: dL/d(blended features) */
     float *d_base_w;              /* [3072] tcnn mlp_base.params layout, += */
@@ -230,6 +239,8 @@ typedef struct nsb_field_bwd_args {
     float *cw_slots_out;          /* NULL or [n_slots][32] out: the effective (fp16-rounded) blend weights of each slot's
                                      timestep, exactly as the expansion uses them -- input of nsb_table_adam_step /
                                      nsb_rank1_expand when the caller defers the table gradient (d_tables == NULL) */
+    float *d_sample_blend_codes;  /* [n][32] out or NULL: with nsb_samples.sample_blend_codes, each sample's blend-code
+                                     gradient (written, not accumulated; direct scatter, d_blend_codes is not touched) */
 } nsb_field_bwd_args;
 int nsb_field_backward(const nsb_field_params *params, const nsb_field_opts *opts, const nsb_samples *samples,
                        const nsb_field_bwd_args *args, void *stream);
@@ -251,6 +262,11 @@ typedef struct nsb_deform_bwd_args {
     float *d_warp_codes;          /* [n_timesteps][128] or NULL */
     void *dw_workspace;           /* nsb_deform_bwd_workspace_bytes() of scratch (need not be zeroed): per-CTA private
                                      weight-gradient accumulators, summed into d_stem_w at the end of the call */
+    /* Per-sample warp codes (component API; the forward took them as nsb_samples.sample_code_bias).  When set, the code
+       columns of d_stem_w[0] / d_stem_w[4] use these codes, params->warp_codes and d_warp_codes are not used, and
+       d_sample_warp_codes (NULL: skip) receives each sample's code gradient, ACCUMULATED (+=) without atomics. */
+    const void *sample_warp_codes;  /* __half [n][128] or NULL */
+    float *d_sample_warp_codes;     /* [n][128] */
 } nsb_deform_bwd_args;
 size_t nsb_deform_packed_t_bytes(void);
 size_t nsb_deform_bwd_workspace_bytes(void);

@@ -55,7 +55,8 @@ class FieldBwdArgs(C.Structure):
                 ("rgb", C.c_void_p), ("d_sigma", C.c_void_p), ("d_rgb", C.c_void_p), ("loss_scale", C.c_float),
                 ("d_feat", C.c_void_p), ("d_base_w", C.c_void_p), ("d_head_w", C.c_void_p), ("d_tables", C.c_void_p),
                 ("d_blend_codes", C.c_void_p), ("d_xs", C.c_void_p), ("g_rank1", C.c_void_p), ("ts_slot", C.c_void_p),
-                ("n_slots", C.c_int32), ("corner_vals", C.c_void_p), ("cw_slots_out", C.c_void_p)]
+                ("n_slots", C.c_int32), ("corner_vals", C.c_void_p), ("cw_slots_out", C.c_void_p),
+                ("d_sample_blend_codes", C.c_void_p)]
 
 
 class TableAdamArgs(C.Structure):
@@ -90,7 +91,8 @@ class DeformBwdArgs(C.Structure):
     _fields_ = [("deform_packed_t", C.c_void_p), ("deform_acts", C.c_void_p), ("deform_enc", C.c_void_p),
                 ("d_xs", C.c_void_p), ("loss_scale", C.c_float), ("d_stem_w", C.c_void_p * 6), ("d_stem_b", C.c_void_p),
                 ("d_r_w", C.c_void_p), ("d_r_b", C.c_void_p), ("d_v_w", C.c_void_p), ("d_v_b", C.c_void_p),
-                ("d_warp_codes", C.c_void_p), ("dw_workspace", C.c_void_p)]
+                ("d_warp_codes", C.c_void_p), ("dw_workspace", C.c_void_p), ("sample_warp_codes", C.c_void_p),
+                ("d_sample_warp_codes", C.c_void_p)]
 
 
 class CompositeBwdArgs(C.Structure):
@@ -166,6 +168,8 @@ SYMBOLS = {
     "nsb_rank1_expand": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_void_p, C.c_void_p]),
     "nsb_hash_blend_forward": (C.c_int, [C.POINTER(FieldParams), C.POINTER(FieldOpts), C.c_void_p, C.c_void_p,
                                          C.c_int64, C.c_void_p, C.c_int32, C.c_void_p]),
+    "nsb_hash_blend_backward": (C.c_int, [C.POINTER(FieldParams), C.POINTER(FieldOpts), C.c_void_p, C.c_void_p,
+                                          C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "nsb_composite_forward": (C.c_int, [C.POINTER(CompositeArgs), C.c_void_p]),
     "nsb_composite_backward": (C.c_int, [C.POINTER(CompositeBwdArgs), C.c_void_p]),
     "nsb_march_fixed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_float, C.c_float,

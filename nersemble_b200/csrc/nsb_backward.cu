@@ -16,6 +16,9 @@
 //   gather; per level one 32-byte load (values, for the time-code gradient) and four 16-byte vector reductions
 //   (red.global.add.v4.f32) into the fp32 gradient line of the table entry.
 #include <algorithm>
+#include <cstddef>
+#include <cstring>
+#include <type_traits>
 
 #include "nsb_common.cuh"
 #include "nsb_gather.cuh"
@@ -23,12 +26,41 @@
 
 namespace nsb {
 
+// nsb_field_bwd_args without its trailing per-sample-code field.  The kernels of the training step take this as their
+// parameter block, so the per-sample-code field appended to the C struct moves none of their parameter offsets (the
+// second parameter of hash_expand_kernel would otherwise shift).
+struct FieldBwdCore {
+    const void *field_packed_t, *feat;
+    const float *xs, *sigma, *rgb, *d_sigma, *d_rgb;
+    float loss_scale;
+    float *d_feat, *d_base_w, *d_head_w, *d_tables, *d_blend_codes, *d_xs, *g_rank1;
+    const int32_t *ts_slot;
+    int32_t n_slots;
+    const void *corner_vals;
+    float *cw_slots_out;
+};
+static_assert(sizeof(FieldBwdCore) == offsetof(nsb_field_bwd_args, d_sample_blend_codes) &&
+              offsetof(FieldBwdCore, loss_scale) == offsetof(nsb_field_bwd_args, loss_scale) &&
+              offsetof(FieldBwdCore, n_slots) == offsetof(nsb_field_bwd_args, n_slots) &&
+              offsetof(FieldBwdCore, cw_slots_out) == offsetof(nsb_field_bwd_args, cw_slots_out),
+              "FieldBwdCore must be the leading part of nsb_field_bwd_args");
+
 struct FieldBwdKArgs {
     nsb_field_params P;
     nsb_field_opts O;
     nsb_samples S;
-    nsb_field_bwd_args B;
+    FieldBwdCore B;
 };
+
+// hash_bwd_kernel modes: blend codes of the time-embedding table (training; the code gradient is summed per timestep),
+// per-sample blend codes (component field: per-sample code gradient), and the stand-alone HashEnsemble (positions are
+// the normalised hash input itself, S.positions [n][3], always in the box; d_feat is the output gradient).
+enum HashBwdMode { kTableCodes = 0, kSampleCodes = 1, kBlendOnly = 2 };
+struct FieldBwdKArgsPS : FieldBwdKArgs {
+    float *d_sample_codes;   // [n][32] or NULL
+};
+template <int MODE>
+using HashBwdKArgs = std::conditional_t<MODE == kTableCodes, FieldBwdKArgs, FieldBwdKArgsPS>;
 
 constexpr int kBaseW = 64 * 32 + 16 * 64;             // 3072
 constexpr int kHeadW = 64 * 32 + 64 * 64 + 16 * 64;   // 7168
@@ -280,7 +312,9 @@ __device__ __forceinline__ void red_add_v4(float *p, float a, float b, float c, 
     asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
 }
 
-__global__ void __launch_bounds__(256) hash_bwd_kernel(const __grid_constant__ FieldBwdKArgs K) {
+template <int MODE>
+__global__ void __launch_bounds__(256) hash_bwd_kernel(const __grid_constant__ HashBwdKArgs<MODE> K) {
+    constexpr bool kPerSample = MODE != kTableCodes;
     const int lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
     const uint32_t dx = g & 1, dy = (g >> 1) & 1, dz = g >> 2;
     const int64_t n = K.S.n_samples;
@@ -304,22 +338,32 @@ __global__ void __launch_bounds__(256) hash_bwd_kernel(const __grid_constant__ F
         for (int j = 0; j < 8; ++j) code_acc[j] = 0.f;
     };
     for (int64_t s = s_begin; s < s_end; ++s) {
-        const float4 xs = __ldg(reinterpret_cast<const float4 *>(K.B.xs) + s);
-        // timestep of the sample (same rounding as the forward)
-        float tt = 0.f;
-        if (K.S.origins != nullptr) { if (K.S.ray_times) tt = K.S.ray_times[K.S.ray_indices[s]]; }
-        else if (K.S.sample_times) tt = K.S.sample_times[s];
-        int ts = __float2int_rn(__fmul_rn(tt, (float)(K.P.n_timesteps - 1)));
-        ts = min(max(ts, 0), K.P.n_timesteps - 1);
-        if (ts != acc_ts) { flush_codes(); acc_ts = ts; }
-        const bool rank1 = K.B.g_rank1 != nullptr;
+        float4 xs;
+        if constexpr (MODE == kBlendOnly)
+            xs = make_float4(K.S.positions[3 * s + 0], K.S.positions[3 * s + 1], K.S.positions[3 * s + 2], 1.0f);
+        else
+            xs = __ldg(reinterpret_cast<const float4 *>(K.B.xs) + s);
+        bool rank1 = false;
         float *gslot = nullptr;
-        if (rank1) {
-            const int slot = K.B.ts_slot[ts];
-            gslot = K.B.g_rank1 + (size_t)slot * ((size_t)K.P.levels.offset[NSB_MAX_LEVELS - 1] + K.P.levels.entries[NSB_MAX_LEVELS - 1]) * 2;
+        const float *code_row;
+        if constexpr (kPerSample) {
+            code_row = K.S.sample_blend_codes + s * NSB_MEMBERS;
+        } else {
+            // timestep of the sample (same rounding as the forward)
+            float tt = 0.f;
+            if (K.S.origins != nullptr) { if (K.S.ray_times) tt = K.S.ray_times[K.S.ray_indices[s]]; }
+            else if (K.S.sample_times) tt = K.S.sample_times[s];
+            int ts = __float2int_rn(__fmul_rn(tt, (float)(K.P.n_timesteps - 1)));
+            ts = min(max(ts, 0), K.P.n_timesteps - 1);
+            if (ts != acc_ts) { flush_codes(); acc_ts = ts; }
+            rank1 = K.B.g_rank1 != nullptr;
+            if (rank1) {
+                const int slot = K.B.ts_slot[ts];
+                gslot = K.B.g_rank1 + (size_t)slot * ((size_t)K.P.levels.offset[NSB_MAX_LEVELS - 1] + K.P.levels.entries[NSB_MAX_LEVELS - 1]) * 2;
+            }
+            code_row = K.S.sample_blend_codes ? K.S.sample_blend_codes + s * NSB_MEMBERS
+                                              : K.P.blend_codes + (size_t)ts * NSB_MEMBERS;
         }
-        const float *code_row = K.S.sample_blend_codes ? K.S.sample_blend_codes + s * NSB_MEMBERS
-                                                       : K.P.blend_codes + (size_t)ts * NSB_MEMBERS;
         const float4 c0 = __ldg(reinterpret_cast<const float4 *>(code_row) + 2 * q);
         const float4 c1 = __ldg(reinterpret_cast<const float4 *>(code_row) + 2 * q + 1);
         const float craw[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
@@ -354,7 +398,10 @@ __global__ void __launch_bounds__(256) hash_bwd_kernel(const __grid_constant__ F
             if (rank1) {   // 2-vector per (timestep, line); member expansion and code gradient happen in hash_expand_kernel
                 if (q == 0 && (g0 != 0.f || g1 != 0.f)) red_add_v2(gslot + entry * 2, g0, g1);
             }
-            if ((K.B.d_blend_codes && !rank1) || K.B.d_xs) {
+            bool want_values;
+            if constexpr (kPerSample) want_values = K.d_sample_codes || K.B.d_xs;
+            else want_values = (K.B.d_blend_codes && !rank1) || K.B.d_xs;
+            if (want_values) {
                 uint32_t v[8];
                 ldg256(tab + entry * 128, v);
                 float pb0 = 0.f, pb1 = 0.f;   // this lane's share of the member-blended corner value
@@ -390,7 +437,24 @@ __global__ void __launch_bounds__(256) hash_bwd_kernel(const __grid_constant__ F
                 K.B.d_xs[3 * s + 0] = ex * xs.w; K.B.d_xs[3 * s + 1] = ey * xs.w; K.B.d_xs[3 * s + 2] = ez * xs.w;
             }
         }
-        if (K.B.d_blend_codes && !rank1) {
+        if constexpr (kPerSample) {
+            if (K.d_sample_codes) {
+                float v[8];
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {   // sum over the 8 corner lanes (lane bits 2..4); cw = code*scale + bias
+                    v[j] = dcw[j];
+                    v[j] += __shfl_xor_sync(0xffffffffu, v[j], 4);
+                    v[j] += __shfl_xor_sync(0xffffffffu, v[j], 8);
+                    v[j] += __shfl_xor_sync(0xffffffffu, v[j], 16);
+                    v[j] *= K.O.cw_scale[8 * q + j];
+                }
+                if (g == 0) {
+                    float4 *dst = reinterpret_cast<float4 *>(K.d_sample_codes + s * NSB_MEMBERS) + 2 * q;
+                    dst[0] = make_float4(v[0], v[1], v[2], v[3]);
+                    dst[1] = make_float4(v[4], v[5], v[6], v[7]);
+                }
+            }
+        } else if (K.B.d_blend_codes && !rank1) {
 #pragma unroll
             for (int j = 0; j < 8; ++j) {   // sum over the 8 corner lanes (lane bits 2..4)
                 float v = dcw[j];
@@ -401,7 +465,7 @@ __global__ void __launch_bounds__(256) hash_bwd_kernel(const __grid_constant__ F
             }
         }
     }
-    flush_codes();
+    if constexpr (!kPerSample) flush_codes();
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -608,6 +672,14 @@ __global__ void __launch_bounds__(kExpWarps * 32) hash_expand_kernel(const __gri
 }
 
 static int g_bwd_sms = 0;
+static void bwd_sms() {
+    if (g_bwd_sms == 0) {
+        int dev = 0;
+        cudaGetDevice(&dev);
+        cudaDeviceGetAttribute(&g_bwd_sms, cudaDevAttrMultiProcessorCount, dev);
+        if (g_bwd_sms <= 0) g_bwd_sms = 132;
+    }
+}
 
 }  // namespace nsb
 
@@ -617,25 +689,27 @@ extern "C" int nsb_field_backward(const nsb_field_params *params, const nsb_fiel
                                   const nsb_field_bwd_args *args, void *stream) {
     if (!params || !opts || !samples || !args) { set_error("nsb_field_backward: null argument"); return 1; }
     if (samples->n_samples <= 0) return 0;
-    if (!args->field_packed_t || !params->field_packed || !args->feat || !args->xs || !args->sigma || !args->rgb ||
-        !args->d_feat || !(args->loss_scale > 0.f)) {
+    if (!args->field_packed_t || !params->field_packed || !args->feat || !args->xs || !args->sigma ||
+        (!args->rgb && args->d_rgb) || !args->d_feat || !(args->loss_scale > 0.f)) {
         set_error("nsb_field_backward: missing saved tensors / workspace / loss_scale");
         return 1;
     }
-    if ((args->d_tables || args->d_blend_codes || args->d_xs) && (!params->tables || (!params->blend_codes && !samples->sample_blend_codes))) {
+    const bool per_sample = args->d_sample_blend_codes != nullptr;
+    const bool hash_pass = args->d_tables || args->d_blend_codes || args->d_xs || per_sample;
+    if (hash_pass && (!params->tables || (!params->blend_codes && !samples->sample_blend_codes))) {
         set_error("nsb_field_backward: tables / blend codes missing");
         return 1;
     }
-    if (params->levels.n_levels != NSB_MAX_LEVELS) { set_error("nsb_field_backward: n_levels must be 16"); return 1; }
-    if (g_bwd_sms == 0) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&g_bwd_sms, cudaDevAttrMultiProcessorCount, dev);
-        if (g_bwd_sms <= 0) g_bwd_sms = 132;
+    if (per_sample && (!samples->sample_blend_codes || args->g_rank1)) {
+        set_error("nsb_field_backward: d_sample_blend_codes needs per-sample blend codes and the direct scatter (no g_rank1)");
+        return 1;
     }
+    if (params->levels.n_levels != NSB_MAX_LEVELS) { set_error("nsb_field_backward: n_levels must be 16"); return 1; }
+    bwd_sms();
     cudaStream_t st = (cudaStream_t)stream;
     FieldBwdKArgs K;
-    K.P = *params; K.O = *opts; K.S = *samples; K.B = *args;
+    K.P = *params; K.O = *opts; K.S = *samples;
+    std::memcpy(&K.B, args, sizeof(FieldBwdCore));
     static bool configured = false;
     {   // 16x16 output blocks of the five weight matrices, in flat-accumulator order (see SmemBwd)
         static bool table_done_dev[64] = {};
@@ -670,8 +744,15 @@ extern "C" int nsb_field_backward(const nsb_field_params *params, const nsb_fiel
     field_mlp_bwd_kernel<<<(int)std::min<int64_t>(n_tiles, g_bwd_sms), 256, smem, st>>>(K);
     int rc = check_launch("field_mlp_bwd_kernel");
     if (rc) return rc;
-    if (args->d_tables || args->d_blend_codes || args->d_xs) {
+    if (hash_pass) {
         const int blocks = (int)std::min<int64_t>((samples->n_samples + 7) / 8, (int64_t)g_bwd_sms * 8);
+        if (per_sample) {
+            FieldBwdKArgsPS KP;
+            static_cast<FieldBwdKArgs &>(KP) = K;
+            KP.d_sample_codes = args->d_sample_blend_codes;
+            hash_bwd_kernel<kSampleCodes><<<blocks, 256, 0, st>>>(KP);
+            return check_launch("hash_bwd_kernel");
+        }
         if (args->g_rank1) {
             if (!args->ts_slot || args->n_slots < 1 || args->n_slots > kMaxSlots || samples->sample_blend_codes) {
                 set_error("nsb_field_backward: rank-1 path needs ts_slot, 1 <= n_slots <= 32 and table-indexed blend codes");
@@ -682,7 +763,7 @@ extern "C" int nsb_field_backward(const nsb_field_params *params, const nsb_fiel
             hash_bwd_cv_kernel<<<blocks, 256, 0, st>>>(K);
             rc = check_launch("hash_bwd_cv_kernel");
         } else {
-            hash_bwd_kernel<<<blocks, 256, 0, st>>>(K);
+            hash_bwd_kernel<kTableCodes><<<blocks, 256, 0, st>>>(K);
             rc = check_launch("hash_bwd_kernel");
         }
         if (rc) return rc;
@@ -694,4 +775,26 @@ extern "C" int nsb_field_backward(const nsb_field_params *params, const nsb_fiel
         }
     }
     return rc;
+}
+
+extern "C" int nsb_hash_blend_backward(const nsb_field_params *params, const nsb_field_opts *opts, const float *x,
+                                       const float *codes, int64_t n, const float *d_out, float *d_tables, float *d_codes,
+                                       float *d_x, void *stream) {
+    if (!params || !opts || !x || !codes || !d_out) { set_error("nsb_hash_blend_backward: null argument"); return 1; }
+    if (n <= 0 || !(d_tables || d_codes || d_x)) return 0;
+    if (!params->tables) { set_error("nsb_hash_blend_backward: tables missing"); return 1; }
+    if (params->levels.n_levels != NSB_MAX_LEVELS) { set_error("nsb_hash_blend_backward: n_levels must be 16"); return 1; }
+    bwd_sms();
+    FieldBwdKArgsPS K = {};
+    K.P = *params; K.O = *opts;
+    K.S.n_samples = n;
+    K.S.positions = x;
+    K.S.sample_blend_codes = codes;
+    K.B.d_feat = const_cast<float *>(d_out);     // read only
+    K.B.d_tables = d_tables;
+    K.B.d_xs = d_x;
+    K.d_sample_codes = d_codes;
+    const int blocks = (int)std::min<int64_t>((n + 7) / 8, (int64_t)g_bwd_sms * 8);
+    hash_bwd_kernel<kBlendOnly><<<blocks, 256, 0, (cudaStream_t)stream>>>(K);
+    return check_launch("hash_bwd_kernel");
 }

@@ -15,18 +15,43 @@
 //     output-row block w of dW_l (movmatrix transposes, K = 8 row blocks) and adds it to the fp32 gradient;
 //   * warp-code gradients = delta . W[:, code columns], summed over the rows of a warp (one ray -> one timestep).
 #include <algorithm>
+#include <cstddef>
+#include <cstring>
+#include <type_traits>
 
 #include "nsb_common.cuh"
 
 namespace nsb {
 
+// nsb_deform_bwd_args without its trailing per-sample-code fields: the table-code kernel keeps its parameter offsets
+// (aabb_size follows B), the per-sample pointers ride after aabb_size in DeformBwdKArgsPS.
+struct DeformBwdCore {
+    const void *deform_packed_t, *deform_acts, *deform_enc;
+    const float *d_xs;
+    float loss_scale;
+    float *d_stem_w[6];
+    float *d_stem_b, *d_r_w, *d_r_b, *d_v_w, *d_v_b, *d_warp_codes;
+    void *dw_workspace;
+};
+static_assert(sizeof(DeformBwdCore) == offsetof(nsb_deform_bwd_args, sample_warp_codes) &&
+              offsetof(DeformBwdCore, loss_scale) == offsetof(nsb_deform_bwd_args, loss_scale) &&
+              offsetof(DeformBwdCore, d_stem_w) == offsetof(nsb_deform_bwd_args, d_stem_w) &&
+              offsetof(DeformBwdCore, dw_workspace) == offsetof(nsb_deform_bwd_args, dw_workspace),
+              "DeformBwdCore must be the leading part of nsb_deform_bwd_args");
+
 struct DeformBwdKArgs {
     nsb_field_params P;
     nsb_field_opts O;
     nsb_samples S;
-    nsb_deform_bwd_args B;
+    DeformBwdCore B;
     float aabb_size[3];
 };
+struct DeformBwdKArgsPS : DeformBwdKArgs {
+    const __half *sample_warp_codes;   // [n][128]
+    float *d_sample_warp_codes;        // [n][128] or NULL
+};
+template <bool PER_SAMPLE>
+using DeformBwdKArgsT = std::conditional_t<PER_SAMPLE, DeformBwdKArgsPS, DeformBwdKArgs>;
 
 constexpr int kDSlab = 2048, kDChunkSlabs = 4, kDChunkBytes = kDSlab * kDChunkSlabs, kDStages = 4;
 // transposed slab order = order of use: heads, L5, L4 (hidden cols), L4 (code cols), L3, L2, L1, L0 (code cols)
@@ -280,8 +305,11 @@ __global__ void __launch_bounds__(256) deform_dw_reduce_kernel(const __grid_cons
 //   DW    warps 8-15 : output block ob = w - 8 of every weight gradient (tile-wide contraction), bias sums
 // (One role per warp doubled the resident warps: the 8-warp version was latency-bound at
 //  12.5 % occupancy, the dX chain and the dW contraction of a layer are independent once D / X are staged.)
+// PER_SAMPLE: the warp codes are per-sample rows (component API) instead of the timestep's row of the embedding, and the
+// code-column gradient of every row is written to its own row of d_sample_warp_codes.
 constexpr int kDbThreads = 512;
-__global__ void __launch_bounds__(kDbThreads, 1) deform_bwd_kernel(const __grid_constant__ DeformBwdKArgs K) {
+template <bool PER_SAMPLE>
+__global__ void __launch_bounds__(kDbThreads, 1) deform_bwd_kernel(const __grid_constant__ DeformBwdKArgsT<PER_SAMPLE> K) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     SmemDB &sm = *reinterpret_cast<SmemDB *>(smem_raw);
     const int tid = threadIdx.x, lane = tid & 31;
@@ -491,16 +519,36 @@ __global__ void __launch_bounds__(kDbThreads, 1) deform_bwd_kernel(const __grid_
                 const int eb = l == 4 ? 8 : 0;   // k-tile offset of [enc | code] inside X
 #pragma unroll
                 for (int kt = 0; kt < 3; ++kt) sm.X[warp][eb + kt][lane] = movt4(__ldcs(enc_w + kt * 32 + lane));
-                const __half *cd0 = reinterpret_cast<const __half *>(K.P.warp_codes) + (size_t)tsr[0] * NSB_WARP_CODE_DIM;
-                const __half *cd1 = reinterpret_cast<const __half *>(K.P.warp_codes) + (size_t)tsr[1] * NSB_WARP_CODE_DIM;
+                if constexpr (PER_SAMPLE) {
+                    // rows past the end stage zeros: their deltas are 0, and 0 x (uninitialised fp16) could be NaN
+                    const int64_t sa = row0 + g, sb = row0 + g + 8;
+                    const __half *cd0 = K.sample_warp_codes + (size_t)sa * NSB_WARP_CODE_DIM;
+                    const __half *cd1 = K.sample_warp_codes + (size_t)sb * NSB_WARP_CODE_DIM;
 #pragma unroll
-                for (int kc = 0; kc < 8; ++kc) {
-                    uint4 cv;
-                    cv.x = __ldg(reinterpret_cast<const uint32_t *>(cd0 + kc * 16 + 2 * q));
-                    cv.y = __ldg(reinterpret_cast<const uint32_t *>(cd1 + kc * 16 + 2 * q));
-                    cv.z = __ldg(reinterpret_cast<const uint32_t *>(cd0 + kc * 16 + 2 * q + 8));
-                    cv.w = __ldg(reinterpret_cast<const uint32_t *>(cd1 + kc * 16 + 2 * q + 8));
-                    sm.X[warp][eb + 3 + kc][lane] = movt4(cv);
+                    for (int kc = 0; kc < 8; ++kc) {
+                        uint4 cv = make_uint4(0u, 0u, 0u, 0u);
+                        if (sa < n) {
+                            cv.x = __ldg(reinterpret_cast<const uint32_t *>(cd0 + kc * 16 + 2 * q));
+                            cv.z = __ldg(reinterpret_cast<const uint32_t *>(cd0 + kc * 16 + 2 * q + 8));
+                        }
+                        if (sb < n) {
+                            cv.y = __ldg(reinterpret_cast<const uint32_t *>(cd1 + kc * 16 + 2 * q));
+                            cv.w = __ldg(reinterpret_cast<const uint32_t *>(cd1 + kc * 16 + 2 * q + 8));
+                        }
+                        sm.X[warp][eb + 3 + kc][lane] = movt4(cv);
+                    }
+                } else {
+                    const __half *cd0 = reinterpret_cast<const __half *>(K.P.warp_codes) + (size_t)tsr[0] * NSB_WARP_CODE_DIM;
+                    const __half *cd1 = reinterpret_cast<const __half *>(K.P.warp_codes) + (size_t)tsr[1] * NSB_WARP_CODE_DIM;
+#pragma unroll
+                    for (int kc = 0; kc < 8; ++kc) {
+                        uint4 cv;
+                        cv.x = __ldg(reinterpret_cast<const uint32_t *>(cd0 + kc * 16 + 2 * q));
+                        cv.y = __ldg(reinterpret_cast<const uint32_t *>(cd1 + kc * 16 + 2 * q));
+                        cv.z = __ldg(reinterpret_cast<const uint32_t *>(cd0 + kc * 16 + 2 * q + 8));
+                        cv.w = __ldg(reinterpret_cast<const uint32_t *>(cd1 + kc * 16 + 2 * q + 8));
+                        sm.X[warp][eb + 3 + kc][lane] = movt4(cv);
+                    }
                 }
             }
             }   // chain: staging
@@ -550,7 +598,26 @@ __global__ void __launch_bounds__(kDbThreads, 1) deform_bwd_kernel(const __grid_
                     float acc[8][4];
                     zero8(acc);
                     tring_gemm(acc, j0 + half * 8, 8, da, sm, rf, lane);
-                    if (K.B.d_warp_codes) {
+                    if constexpr (PER_SAMPLE) {
+                        // this lane owns columns col, col+1 of rows g / g+8 for layers 4 and 0 alike: plain +=, no atomics
+                        if (K.d_sample_warp_codes) {
+                            const int64_t sa = row0 + g, sb = row0 + g + 8;
+#pragma unroll
+                            for (int nt = 0; nt < 8; ++nt) {
+                                const int col = half * 64 + nt * 8 + 2 * q;
+                                if (sa < n) {
+                                    float2 *p = reinterpret_cast<float2 *>(K.d_sample_warp_codes + (size_t)sa * NSB_WARP_CODE_DIM + col);
+                                    const float2 v = *p;
+                                    *p = make_float2(v.x + acc[nt][0] * inv_ls, v.y + acc[nt][1] * inv_ls);
+                                }
+                                if (sb < n) {
+                                    float2 *p = reinterpret_cast<float2 *>(K.d_sample_warp_codes + (size_t)sb * NSB_WARP_CODE_DIM + col);
+                                    const float2 v = *p;
+                                    *p = make_float2(v.x + acc[nt][2] * inv_ls, v.y + acc[nt][3] * inv_ls);
+                                }
+                            }
+                        }
+                    } else if (K.B.d_warp_codes) {
 #pragma unroll
                         for (int nt = 0; nt < 8; ++nt) {
                             const int col = half * 64 + nt * 8 + 2 * q;
@@ -611,35 +678,48 @@ static int db_sms() {
 
 extern "C" size_t nsb_deform_bwd_workspace_bytes(void) { return (size_t)db_sms() * kScrF4 * sizeof(float4); }
 
+template <bool PER_SAMPLE>
+static int launch_deform_bwd(const DeformBwdKArgsPS &K, int n_ctas, size_t smem, cudaStream_t st) {
+    static bool configured = false;
+    if (!configured) {
+        cudaError_t e = cudaFuncSetAttribute(deform_bwd_kernel<PER_SAMPLE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(deform_bwd_kernel): %s", cudaGetErrorString(e)); return 1; }
+        configured = true;
+    }
+    deform_bwd_kernel<PER_SAMPLE><<<n_ctas, kDbThreads, smem, st>>>(static_cast<const DeformBwdKArgsT<PER_SAMPLE> &>(K));
+    return check_launch("deform_bwd_kernel");
+}
+
 extern "C" int nsb_deform_backward(const nsb_field_params *params, const nsb_field_opts *opts, const nsb_samples *samples,
                                    const nsb_deform_bwd_args *args, void *stream) {
     if (!params || !opts || !samples || !args) { set_error("nsb_deform_backward: null argument"); return 1; }
     if (samples->n_samples <= 0) return 0;
+    const bool per_sample = args->sample_warp_codes != nullptr;
     if (!args->deform_packed_t || !args->deform_acts || !args->deform_enc || !args->d_xs || !params->deform_packed_tb ||
-        !params->deform_bias || !params->warp_codes || !(args->loss_scale > 0.f) || !args->d_stem_b || !args->d_r_w ||
-        !args->d_r_b || !args->d_v_w || !args->d_v_b) {
+        !params->deform_bias || (!params->warp_codes && !per_sample) || !(args->loss_scale > 0.f) || !args->d_stem_b ||
+        !args->d_r_w || !args->d_r_b || !args->d_v_w || !args->d_v_b) {
         set_error("nsb_deform_backward: missing tensors");
         return 1;
     }
     for (int l = 0; l < 6; ++l)
         if (!args->d_stem_w[l]) { set_error("nsb_deform_backward: d_stem_w[%d] missing", l); return 1; }
-    if (samples->sample_code_bias) { set_error("nsb_deform_backward: per-sample warp codes are not supported"); return 1; }
+    if (samples->sample_code_bias && !per_sample) {
+        set_error("nsb_deform_backward: a per-sample code bias needs the per-sample warp codes (sample_warp_codes)");
+        return 1;
+    }
     if (!args->dw_workspace) { set_error("nsb_deform_backward: dw_workspace missing (nsb_deform_bwd_workspace_bytes)"); return 1; }
     db_sms();
-    DeformBwdKArgs K;
-    K.P = *params; K.O = *opts; K.S = *samples; K.B = *args;
+    DeformBwdKArgsPS K;
+    K.P = *params; K.O = *opts; K.S = *samples;
+    std::memcpy(&K.B, args, sizeof(DeformBwdCore));
     for (int k = 0; k < 3; ++k) K.aabb_size[k] = params->aabb[3 + k] - params->aabb[k];
-    static bool configured = false;
+    K.sample_warp_codes = reinterpret_cast<const __half *>(args->sample_warp_codes);
+    K.d_sample_warp_codes = args->d_sample_warp_codes;
     const size_t smem = sizeof(SmemDB);
-    if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(deform_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(deform_bwd_kernel): %s", cudaGetErrorString(e)); return 1; }
-        configured = true;
-    }
     const int64_t n_tiles = (samples->n_samples + NSB_TILE - 1) / NSB_TILE;
     const int n_ctas = (int)std::min<int64_t>(n_tiles, g_db_sms);
-    deform_bwd_kernel<<<n_ctas, kDbThreads, smem, (cudaStream_t)stream>>>(K);
-    int rc = check_launch("deform_bwd_kernel");
+    int rc = per_sample ? launch_deform_bwd<true>(K, n_ctas, smem, (cudaStream_t)stream)
+                        : launch_deform_bwd<false>(K, n_ctas, smem, (cudaStream_t)stream);
     if (rc) return rc;
     DwReduceArgs R;
     R.scratch = reinterpret_cast<const float4 *>(args->dw_workspace);

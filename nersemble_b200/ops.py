@@ -364,14 +364,16 @@ def field_backward(P: NativeParams, saved: Dict[str, torch.Tensor], d_sigma: Opt
                    **sample_kw) -> Dict[str, torch.Tensor]:
     """Backward of the density/colour MLPs and the hash ensemble (nsb_field_backward).
     saved: feat, xs, sigma, rgb from field_forward(want=(..., "feat", "xs")).  Returns fp32 gradients:
-    d_base_w [3072], d_head_w [7168] (tcnn flat layouts), d_tables [entries,32,2], d_blend_codes [T,32], d_feat."""
+    d_base_w [3072], d_head_w [7168] (tcnn flat layouts), d_tables [entries,32,2], d_blend_codes [T,32], d_feat.
+    With sample_blend_codes (per-sample conditioning, component API) the code gradient is d_sample_blend_codes [n,32]
+    instead of d_blend_codes, and the table gradient takes the direct scatter."""
     lib = _lib.load()
     keep = []
     s = _lib.Samples()
     n = _fill_samples(s, keep, **sample_kw)
     dev = saved["feat"].device
     a = _lib.FieldBwdArgs()
-    feat = saved["feat"].contiguous(); xs = _f32c(saved["xs"]); sg = _f32c(saved["sigma"]); cc = _f32c(saved["rgb"])
+    feat = saved["feat"].contiguous(); xs = _f32c(saved["xs"]); sg = _f32c(saved["sigma"]); cc = _f32c(saved.get("rgb"))
     dsg = None if d_sigma is None else _f32c(d_sigma).reshape(-1)
     drg = None if d_rgb is None else _f32c(d_rgb).reshape(-1, 3)
     _need_cuda(feat, xs, sg, cc, dsg, drg)
@@ -390,7 +392,10 @@ def field_backward(P: NativeParams, saved: Dict[str, torch.Tensor], d_sigma: Opt
     if want_tables and not defer:
         out["d_tables"] = torch.zeros((P.levels["total_entries"], 32, 2), dtype=_F32, device=dev)
         a.d_tables = _ptr(out["d_tables"])
-    if want_codes:
+    if want_codes and sample_kw.get("sample_blend_codes") is not None:
+        out["d_sample_blend_codes"] = _rows(n, (32,), _F32, dev)     # written for every sample by the kernel
+        a.d_sample_blend_codes = _ptr(out["d_sample_blend_codes"])
+    elif want_codes:
         out["d_blend_codes"] = torch.zeros((P.n_timesteps, 32), dtype=_F32, device=dev)
         a.d_blend_codes = _ptr(out["d_blend_codes"])
     if want_dx:
@@ -534,10 +539,13 @@ def losses_backward(state: dict, upstream: torch.Tensor):
 
 
 def deform_backward(P: NativeParams, saved: Dict[str, torch.Tensor], d_xs: torch.Tensor, *, window_deform=None,
-                    loss_scale: float = 128.0, **sample_kw) -> Dict[str, torch.Tensor]:
+                    loss_scale: float = 128.0, sample_warp_codes: Optional[torch.Tensor] = None,
+                    **sample_kw) -> Dict[str, torch.Tensor]:
     """Backward of the SE(3) deformation field (nsb_deform_backward).  saved: deform_acts, deform_enc from
     field_forward(want=(..., "deform_acts")); d_xs from field_backward(want_dx=True).  Returns fp32 gradients in
-    the reference layouts: d_stem_w (list of 6), d_stem_b [6,128], d_r_w, d_r_b, d_v_w, d_v_b, d_warp_codes [T,128]."""
+    the reference layouts: d_stem_w (list of 6), d_stem_b [6,128], d_r_w, d_r_b, d_v_w, d_v_b, d_warp_codes [T,128].
+    sample_warp_codes [n,128]: the per-sample codes the forward was given (component API); the code gradient is then
+    d_sample_warp_codes [n,128] instead of d_warp_codes."""
     lib = _lib.load()
     keep = []
     s = _lib.Samples()
@@ -545,6 +553,7 @@ def deform_backward(P: NativeParams, saved: Dict[str, torch.Tensor], d_xs: torch
     dev = d_xs.device
     a = _lib.DeformBwdArgs()
     dxs = _f32c(d_xs).reshape(-1, 3)
+    _need_cuda(dxs, sample_warp_codes)
     a.deform_packed_t = _ptr(P.deform_packed_t)
     a.deform_acts, a.deform_enc, a.d_xs = _ptr(saved["deform_acts"]), _ptr(saved["deform_enc"]), _ptr(dxs)
     a.loss_scale = float(loss_scale)
@@ -552,12 +561,20 @@ def deform_backward(P: NativeParams, saved: Dict[str, torch.Tensor], d_xs: torch
     out = {"d_stem_w": [torch.zeros(d, dtype=_F32, device=dev) for d in dims],
            "d_stem_b": torch.zeros((6, 128), dtype=_F32, device=dev),
            "d_r_w": torch.zeros((3, 128), dtype=_F32, device=dev), "d_r_b": torch.zeros((3,), dtype=_F32, device=dev),
-           "d_v_w": torch.zeros((3, 128), dtype=_F32, device=dev), "d_v_b": torch.zeros((3,), dtype=_F32, device=dev),
-           "d_warp_codes": torch.zeros((P.n_timesteps, 128), dtype=_F32, device=dev)}
+           "d_v_w": torch.zeros((3, 128), dtype=_F32, device=dev), "d_v_b": torch.zeros((3,), dtype=_F32, device=dev)}
     for l in range(6):
         a.d_stem_w[l] = _ptr(out["d_stem_w"][l])
     a.d_stem_b, a.d_r_w, a.d_r_b = _ptr(out["d_stem_b"]), _ptr(out["d_r_w"]), _ptr(out["d_r_b"])
-    a.d_v_w, a.d_v_b, a.d_warp_codes = _ptr(out["d_v_w"]), _ptr(out["d_v_b"]), _ptr(out["d_warp_codes"])
+    a.d_v_w, a.d_v_b = _ptr(out["d_v_w"]), _ptr(out["d_v_b"])
+    if sample_warp_codes is not None:
+        assert sample_warp_codes.shape == (n, 128)
+        swc = sample_warp_codes.detach().to(torch.float16).contiguous()      # the fp16 operand the forward used
+        keep.append(swc)
+        out["d_sample_warp_codes"] = _rows(n, (128,), _F32, dev, zero=True)
+        a.sample_warp_codes, a.d_sample_warp_codes = _ptr(swc), _ptr(out["d_sample_warp_codes"])
+    else:
+        out["d_warp_codes"] = torch.zeros((P.n_timesteps, 128), dtype=_F32, device=dev)
+        a.d_warp_codes = _ptr(out["d_warp_codes"])
     ws = _workspace("deform_bwd", int(lib.nsb_deform_bwd_workspace_bytes()), dev)
     a.dw_workspace = _ptr(ws)
     if n == 0:
@@ -582,6 +599,33 @@ def hash_blend_forward(P: NativeParams, x: torch.Tensor, codes: torch.Tensor, wi
     cp = P.c_params()
     rc = lib.nsb_hash_blend_forward(C.byref(cp), C.byref(opts), _ptr(x), _ptr(codes), n, _ptr(out), int(out_half), _stream())
     _lib.check(rc, "nsb_hash_blend_forward")
+    return out
+
+
+def hash_blend_backward(P: NativeParams, x: torch.Tensor, codes: torch.Tensor, d_out: torch.Tensor, window_hash=None,
+                        want_tables: bool = True, want_codes: bool = True, want_dx: bool = True, disable_initial=True,
+                        soft_transition=True) -> Dict[str, torch.Tensor]:
+    """Backward of hash_blend_forward (nsb_hash_blend_backward) for d_out [n,32]: fp32 d_tables [entries,32,2] (dense),
+    d_codes [n,32], d_x [n,3] -- each only when wanted."""
+    lib = _lib.load()
+    x = _f32c(x); codes = _f32c(codes); d_out = _f32c(d_out)
+    _need_cuda(x, codes, d_out)
+    n, dev = x.shape[0], x.device
+    assert codes.shape == (n, 32) and d_out.shape == (n, 32)
+    out = {}
+    if want_tables:
+        out["d_tables"] = torch.zeros((P.levels["total_entries"], 32, 2), dtype=_F32, device=dev)
+    if want_codes:
+        out["d_codes"] = torch.empty((n, 32), dtype=_F32, device=dev)
+    if want_dx:
+        out["d_x"] = torch.empty((n, 3), dtype=_F32, device=dev)
+    if n == 0:
+        return out
+    opts = make_opts(window_hash, None, False, False, disable_initial, soft_transition)
+    cp = P.c_params()
+    rc = lib.nsb_hash_blend_backward(C.byref(cp), C.byref(opts), _ptr(x), _ptr(codes), n, _ptr(d_out),
+                                     _ptr(out.get("d_tables")), _ptr(out.get("d_codes")), _ptr(out.get("d_x")), _stream())
+    _lib.check(rc, "nsb_hash_blend_backward")
     return out
 
 

@@ -11,15 +11,36 @@ from typing import Dict, List, Literal, Optional, Tuple
 
 import torch
 from torch import nn
+from torch.autograd.function import once_differentiable
 
 from .. import ops, packing
 
 
-def _no_autograd(*tensors):
-    if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tensors):
-        raise NotImplementedError(
-            "the stand-alone component modules are forward-only: gradients flow through the fused model path "
-            "(NeRSembleNGPModel.get_outputs in training mode); wrap this call in torch.no_grad().")
+def _needs_grad(*tensors) -> bool:
+    """True when autograd has to record the call; otherwise the component runs its forward-only path."""
+    return torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tensors)
+
+
+class _HashEnsembleFunction(torch.autograd.Function):
+    """HashEnsemble.forward with gradients for the tables (dense fp32 `.grad`), the conditioning code and the input
+    position: nsb_hash_blend_forward / nsb_hash_blend_backward."""
+
+    @staticmethod
+    def forward(ctx, he, in_tensor, conditioning_code, tables, window):
+        P = he._blend_params()
+        out = ops.hash_blend_forward(P, in_tensor, conditioning_code, window_hash=window, out_half=True, **he._blend_opts())
+        ctx.he, ctx.P, ctx.window = he, P, window
+        ctx.save_for_backward(in_tensor, conditioning_code)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_out):
+        x, code = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        g = ops.hash_blend_backward(ctx.P, x, code, g_out, window_hash=ctx.window, want_tables=need[3],
+                                    want_codes=need[2], want_dx=need[1], **ctx.he._blend_opts())
+        return (None, g.get("d_x"), g.get("d_codes"), g.get("d_tables"), None)
 
 
 class GenericScheduler(nn.Module):
@@ -195,12 +216,17 @@ class HashEnsemble(nn.Module):
         assert conditioning_code.shape[-1] == self.n_hash_encodings, \
             "If blend mixing type is chosen, conditioning code needs to have as many dimensions as there are " \
             "hashtables in the encoding"
-        _no_autograd(in_tensor, conditioning_code, self.tables)
-        P = ops.NativeParams(self.native_tables(), None, None, None, None, torch.tensor([[0., 0, 0], [1, 1, 1]]),
-                             self.levels, 1)
-        return ops.hash_blend_forward(P, in_tensor, conditioning_code, window_hash=window_hash_encodings, out_half=True,
-                                      disable_initial=self.disable_initial_hash_ensemble,
-                                      soft_transition=self.use_soft_transition)
+        if _needs_grad(in_tensor, conditioning_code, self.tables):
+            return _HashEnsembleFunction.apply(self, in_tensor, conditioning_code, self.tables, window_hash_encodings)
+        return ops.hash_blend_forward(self._blend_params(), in_tensor, conditioning_code, window_hash=window_hash_encodings,
+                                      out_half=True, **self._blend_opts())
+
+    def _blend_params(self) -> ops.NativeParams:
+        return ops.NativeParams(self.native_tables(), None, None, None, None, torch.tensor([[0., 0, 0], [1, 1, 1]]),
+                                self.levels, 1)
+
+    def _blend_opts(self) -> dict:
+        return dict(disable_initial=self.disable_initial_hash_ensemble, soft_transition=self.use_soft_transition)
 
     def get_out_dim(self) -> int:
         return self.n_output_dims
@@ -251,6 +277,35 @@ class SE3WarpingField(nn.Module):
                     v_w=self.mlp_v.layers[0].weight, v_b=self.mlp_v.layers[0].bias)
 
 
+class _DeformationFunction(torch.autograd.Function):
+    """SE3DeformationField.compute_offsets with gradients for every se3_field parameter and the per-sample warp codes:
+    nsb_field_forward (deformation only, saving the stem activations) / nsb_deform_backward."""
+
+    @staticmethod
+    def forward(ctx, field, positions, warp_code, window, *params):
+        P = field._native_params()
+        out = ops.field_forward(P, window_hash=None, window_deform=window, use_deformation=True, positions=positions,
+                                sample_warp_codes=warp_code, want=("offsets", "deform_acts"))
+        ctx.field, ctx.P, ctx.window = field, P, window
+        ctx.saved = {"deform_acts": out["deform_acts"], "deform_enc": out["deform_enc"]}
+        ctx.save_for_backward(positions, warp_code)
+        return out["offsets"]
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_offsets):
+        positions, warp_code = ctx.saved_tensors
+        aabb = ctx.field.aabb.detach()
+        d_xs = g_offsets.float() * (aabb[1] - aabb[0]).to(g_offsets.device)   # the offset enters the hash input as offset / size
+        g = ops.deform_backward(ctx.P, ctx.saved, d_xs, window_deform=ctx.window, positions=positions,
+                                sample_warp_codes=warp_code, loss_scale=float(ctx.field.mlp_loss_scale))
+        grads = []
+        for l in range(6):
+            grads += [g["d_stem_w"][l], g["d_stem_b"][l]]
+        grads += [g["d_r_w"], g["d_r_b"], g["d_v_w"], g["d_v_b"]]
+        return (None, None, g["d_sample_warp_codes"], None) + tuple(grads)
+
+
 class SE3DeformationField(nn.Module):
     """deformation_field.py:119-166."""
 
@@ -260,6 +315,7 @@ class SE3DeformationField(nn.Module):
         self.aabb = nn.Parameter(aabb, requires_grad=False)
         self.se3_field = SE3WarpingField(deformation_field_config)
         self.max_n_samples_per_batch = max_n_samples_per_batch   # kept for config compatibility; no chunking needed
+        self.mlp_loss_scale = 128.0      # the backward's fp16 MLP deltas are scaled by this and the gradients divided back
         self._native = None
         self._native_version = None
 
@@ -285,8 +341,21 @@ class SE3DeformationField(nn.Module):
         """Offsets p' - p in NORMALISED aabb units (deformation_field.py:148-166)."""
         if warp_code is None:
             raise TypeError("warp_code is required (the reference would fail on `None - tensor`, deformation_field.py:162)")
-        _no_autograd(positions, warp_code, *self.parameters())
-        P = self._native_params()
-        out = ops.field_forward(P, window_hash=None, window_deform=windows_param, use_deformation=True,
+        params = self._grad_params()
+        if _needs_grad(positions, warp_code, *params):
+            if positions.requires_grad:
+                raise NotImplementedError(
+                    "SE3DeformationField.compute_offsets: gradients w.r.t. the input positions (through the positional "
+                    "encoding) are not implemented; detach the positions.  Parameters and warp codes get gradients.")
+            return _DeformationFunction.apply(self, positions, warp_code, windows_param, *params)
+        out = ops.field_forward(self._native_params(), window_hash=None, window_deform=windows_param, use_deformation=True,
                                 positions=positions, sample_warp_codes=warp_code, want=("offsets",))
         return out["offsets"]
+
+    def _grad_params(self) -> List[nn.Parameter]:
+        """Parameters in the order _DeformationFunction returns their gradients."""
+        f = self.se3_field
+        ps = []
+        for layer in f.mlp_stem.layers:
+            ps += [layer.weight, layer.bias]
+        return ps + [f.mlp_r.layers[0].weight, f.mlp_r.layers[0].bias, f.mlp_v.layers[0].weight, f.mlp_v.layers[0].bias]

@@ -6,13 +6,50 @@ from typing import Dict, Optional, Tuple
 
 import torch
 from torch import Tensor, nn
+from torch.autograd.function import once_differentiable
 
 from .. import ops, packing
 from ..nerfstudio_shim import FieldHeadNames, Frustums, RaySamples
-from .components import HashEnsemble, HashEnsembleConfig, _FlatParams, _no_autograd
+from .components import HashEnsemble, HashEnsembleConfig, _FlatParams, _needs_grad
 
 BASE_SHAPES = [(64, 32), (16, 64)]                 # tcnn mlp_base: 32 -> 64 -> 16 (1 + 15 geo feats)
 HEAD_SHAPES = [(64, 32), (64, 64), (16, 64)]       # tcnn mlp_head: 18 (pad 32 with 1.0) -> 64 -> 64 -> 3 (pad 16)
+
+
+class _FieldFunction(torch.autograd.Function):
+    """density_fn / forward of the field with gradients for mlp_base.params, mlp_head.params, the hash tables (dense
+    fp32 `.grad`), the per-sample time codes and the positions: nsb_field_forward (saving the blended features and the
+    normalised positions) / nsb_field_backward.  Returns (sigma [n], rgb [n,3] or None)."""
+
+    @staticmethod
+    def forward(ctx, field, positions, directions, time_codes, window, want_rgb, base_params, head_params, tables):
+        P = field._native_params()
+        want = ("sigma", "rgb") if want_rgb else ("sigma",)
+        out = ops.field_forward(P, window_hash=window, use_deformation=False, positions=positions,
+                                sample_directions=directions, sample_blend_codes=time_codes, want=want + ("feat", "xs"),
+                                **field._opts())
+        ctx.field, ctx.P, ctx.window = field, P, window
+        ctx.saved = {k: out.get(k) for k in ("feat", "xs", "sigma", "rgb")}    # rgb: None for the density alone
+        ctx.save_for_backward(positions, directions, time_codes)
+        if want_rgb:
+            return out["sigma"], out["rgb"]
+        return out["sigma"], None
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_sigma, g_rgb):
+        positions, directions, time_codes = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        g = ops.field_backward(ctx.P, ctx.saved, g_sigma, g_rgb, window_hash=ctx.window,
+                               loss_scale=float(ctx.field.mlp_loss_scale), want_tables=need[8], want_codes=need[3],
+                               want_dx=need[1], rank1=False, positions=positions, sample_directions=directions,
+                               sample_blend_codes=time_codes, **ctx.field._opts())
+        d_pos = None
+        if need[1]:     # dL/d(world position) = dL/d(normalised position) / aabb size; 0 outside the box (kernel selector)
+            aabb = ctx.field.aabb.detach().float()
+            d_pos = g["d_xs"] / (aabb[1] - aabb[0])
+        return (None, d_pos, None, g.get("d_sample_blend_codes"), None, None, g["d_base_w"], g["d_head_w"],
+                g.get("d_tables"))
 
 
 def _xavier_flat(shapes, gen):
@@ -65,6 +102,7 @@ class NeRSembleNeRFactoField(nn.Module):
             g.manual_seed(seed + 1)
         self.mlp_base = _FlatParams(_xavier_flat(BASE_SHAPES, g))
         self.mlp_head = _FlatParams(_xavier_flat(HEAD_SHAPES, g))
+        self.mlp_loss_scale = 128.0      # the backward's fp16 MLP deltas are scaled by this and the gradients divided back
         self._native = None
         self._native_version = None
 
@@ -90,11 +128,18 @@ class NeRSembleNeRFactoField(nn.Module):
         he = self.hash_ensemble
         return dict(disable_initial=he.disable_initial_hash_ensemble, soft_transition=he.use_soft_transition)
 
+    def _grad_params(self):
+        """The parameters _FieldFunction returns gradients for, in its input order."""
+        return [self.mlp_base.params, self.mlp_head.params, self.hash_ensemble.tables]
+
     # ---- reference API
     def density_fn(self, positions: Tensor, times: Optional[Tensor] = None, window_hash_encodings: Optional[float] = None,
                    time_codes: Optional[Tensor] = None) -> Tensor:
         """nersemble_nerfacto_field.py:228-248."""
-        _no_autograd(positions, time_codes)
+        if _needs_grad(positions, time_codes, *self._grad_params()):
+            sigma, _ = _FieldFunction.apply(self, positions, None, time_codes, window_hash_encodings, False,
+                                            *self._grad_params())
+            return sigma[:, None]
         out = ops.field_forward(self._native_params(), window_hash=window_hash_encodings, use_deformation=False,
                                 positions=positions, sample_blend_codes=time_codes, want=("sigma",), **self._opts())
         return out["sigma"][:, None]
@@ -117,7 +162,10 @@ class NeRSembleNeRFactoField(nn.Module):
             raise AttributeError("Camera indices are not provided.")
         tc = ray_samples.metadata["time_codes"]
         pos = ray_samples.frustums.get_positions()
-        _no_autograd(pos, tc)
+        if _needs_grad(pos, tc, *self._grad_params()):
+            sigma, rgb = _FieldFunction.apply(self, pos, ray_samples.frustums.directions, tc, window_hash_encodings, True,
+                                              *self._grad_params())
+            return {FieldHeadNames.RGB: rgb, FieldHeadNames.DENSITY: sigma[:, None]}
         out = ops.field_forward(self._native_params(), window_hash=window_hash_encodings, use_deformation=False,
                                 positions=pos, sample_directions=ray_samples.frustums.directions, sample_blend_codes=tc,
                                 want=("sigma", "rgb"), **self._opts())

@@ -12,8 +12,7 @@ from torch.nn import Parameter, init
 from .. import ops
 from ..nerfstudio_shim import (FieldHeadNames, Model, RayBundle, RaySamples, SceneBox, TrainingCallback,
                                TrainingCallbackAttributes, TrainingCallbackLocation)
-from .components import (GenericScheduler, HashEnsembleConfig, SE3DeformationField, SE3DeformationFieldConfig,
-                         _no_autograd)
+from .components import GenericScheduler, HashEnsembleConfig, SE3DeformationField, SE3DeformationFieldConfig
 from .field import NeRSembleNeRFactoField
 from .sampler import NeRSembleVolumetricSampler, OccGridEstimator
 
