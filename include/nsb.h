@@ -416,6 +416,30 @@ typedef struct nsb_render_ws_header {  /* first 64 bytes of the workspace; n_tot
 size_t nsb_render_workspace_bytes(int64_t n_rays);
 int nsb_render_forward(const nsb_field_params *params, const nsb_field_opts *opts, const nsb_render_args *args, void *stream);
 
+/* Surface normals of the density field (nerfstudio Field.get_normals, used by NeRSembleNeRFactoField.forward with
+ * compute_normals=True: nerfstudio/fields/nersemble_nerfacto_field.py:385-402) and their per-ray composite
+ * (NormalsRenderer with normalize=True), for samples the field or render kernels already evaluated:
+ *   n = -normalize(grad_scale * d h0 / d x),  normalize(v) = v / max(|v|, 1e-12)
+ * h0 = mlp_base output 0 before trunc_exp; x = the normalised hash-input position after the in-box selector (0 outside
+ * the box: such a sample gets the gradient at the box origin), formed exactly as the field kernels form it (with offsets,
+ * the normalised offsets added to the world position).  With deformation these are canonical-space normals.  The gather
+ * reads the tables the field kernels read for the same params / samples: frame_table (one frame or a timestep stack),
+ * else the 128 B lines with sample_blend_codes or the timestep's blend codes.  Not differentiable.
+ *   out_normals[r] = v / (|v| + 1e-10), v = sum over the ray's packed_info segment of weights[i] * normals[i], summed
+ * in a fixed order (bit-identical from run to run).  Samples beyond *n_samples_dev (when given) are not touched. */
+typedef struct {
+    const float *offsets;        /* [n][3] or NULL (no deformation): the offsets the field / render kernels wrote */
+    float grad_scale[3];          /* per-axis factor on d h0 / d x before normalising: 1 (normalised space, the field API)
+                                     or 1 / aabb extent (world space, rendered normals) */
+    const int64_t *packed_info;   /* [n_rays][2] (start, count), needed for out_normals */
+    int64_t n_rays;
+    const float *weights;         /* [n] render weights, needed for out_normals */
+    float *normals;               /* [n][3] out; NULL: nothing is computed (required for out_normals) */
+    float *out_normals;           /* [n_rays][3] out or NULL */
+} nsb_normals_args;
+int nsb_normals_forward(const nsb_field_params *params, const nsb_field_opts *opts, const nsb_samples *samples,
+                        const nsb_normals_args *args, void *stream);
+
 /* Training sampler WITHOUT host synchronisation (model_components/nersemble_volumetric_sampler.py:95-108 around nerfacc
  * OccGridEstimator.sampling): (1) nsb_march_occupancy_packed = count/scan/fill of nsb_march_occupancy as ONE cooperative
  * launch, the candidate count stays in the workspace header; (2) the caller evaluates the candidates' density with

@@ -141,6 +141,11 @@ class RayBatchArgs(C.Structure):
                 ("out_image", C.c_void_p), ("out_alpha", C.c_void_p), ("out_depth", C.c_void_p)]
 
 
+class NormalsArgs(C.Structure):     # nsb_normals_args
+    _fields_ = [("offsets", C.c_void_p), ("grad_scale", C.c_float * 3), ("packed_info", C.c_void_p), ("n_rays", C.c_int64),
+                ("weights", C.c_void_p), ("normals", C.c_void_p), ("out_normals", C.c_void_p)]
+
+
 class RenderWsHeader(C.Structure):
     _fields_ = [("barrier", C.c_uint32), ("depth_range", C.c_uint32 * 2), ("status", C.c_int32), ("n_total", C.c_int64),
                 ("reserved", C.c_int64 * 5)]
@@ -186,6 +191,8 @@ SYMBOLS = {
     "nsb_visibility_compact": (C.c_int, [C.POINTER(VisCompactArgs), C.c_void_p]),
     "nsb_vis_compact_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64]),
     "nsb_render_forward": (C.c_int, [C.POINTER(FieldParams), C.POINTER(FieldOpts), C.POINTER(RenderArgs), C.c_void_p]),
+    "nsb_normals_forward": (C.c_int, [C.POINTER(FieldParams), C.POINTER(FieldOpts), C.POINTER(Samples),
+                                      C.POINTER(NormalsArgs), C.c_void_p]),
 }
 
 _lib = None

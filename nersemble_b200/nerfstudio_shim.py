@@ -74,6 +74,7 @@ except Exception:  # noqa: BLE001
     class FieldHeadNames(Enum):
         RGB = "rgb"
         DENSITY = "density"
+        NORMALS = "normals"
 
     class TrainingCallbackLocation(Enum):
         BEFORE_TRAIN_ITERATION = auto()

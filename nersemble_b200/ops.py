@@ -332,6 +332,76 @@ def field_forward(P: NativeParams, *, window_hash=None, window_deform=None, use_
     return out
 
 
+def _world_grad_scale(P: NativeParams):
+    """Per-axis factor that turns d h0 / d(normalised position) into d h0 / d(world position): 1 / aabb extent."""
+    a = P.aabb_list
+    return [1.0 / (a[3 + k] - a[k]) for k in range(3)]
+
+
+def _normals_launch(P: NativeParams, cp, opts, s, n_samples: int, dev, *, offsets=None, grad_scale=(1.0, 1.0, 1.0),
+                    packed_info=None, weights=None, keep=None) -> Dict[str, torch.Tensor]:
+    """nsb_normals_forward on filled nsb_samples: per-sample normals [n, 3], and with packed_info / weights the per-ray
+    composite `ray_normals` [R, 3]."""
+    a = _lib.NormalsArgs()
+    keep = list(keep or [])
+    if offsets is not None:
+        offsets = _f32c(offsets).reshape(-1, 3)
+        _need_cuda(offsets)
+        a.offsets = _ptr(offsets); keep.append(offsets)
+    for k in range(3):
+        a.grad_scale[k] = float(grad_scale[k])
+    out = {"normals": _rows(n_samples, (3,), _F32, dev)}
+    a.normals = _ptr(out["normals"])
+    if packed_info is not None:
+        packed_info = packed_info.to(torch.int64).contiguous()
+        weights = _f32c(weights).reshape(-1)
+        _need_cuda(packed_info, weights)
+        keep += [packed_info, weights]
+        R = int(packed_info.shape[0])
+        out["ray_normals"] = torch.zeros((R, 3), dtype=_F32, device=dev)
+        a.packed_info, a.n_rays, a.weights, a.out_normals = _ptr(packed_info), R, _ptr(weights), _ptr(out["ray_normals"])
+    if n_samples > 0:
+        _lib.check(_lib.load().nsb_normals_forward(C.byref(cp), C.byref(opts), C.byref(s), C.byref(a), _stream()),
+                   "nsb_normals_forward")
+    return out
+
+
+def field_normals(P: NativeParams, *, window_hash=None, offsets: Optional[torch.Tensor] = None,
+                  origins=None, directions=None, ray_times=None, t_starts=None, t_ends=None, ray_indices=None,
+                  positions=None, sample_times=None, sample_blend_codes=None, n_samples_dev: Optional[torch.Tensor] = None,
+                  uniform_time: Optional[float] = None, line_gather: bool = False, world_space: bool = False,
+                  packed_info: Optional[torch.Tensor] = None, weights: Optional[torch.Tensor] = None,
+                  disable_initial: bool = True, soft_transition: bool = True) -> Dict[str, torch.Tensor]:
+    """Surface normals of the density field (nsb_normals_forward), nerfstudio's Field.get_normals:
+    n = -normalize(d h0 / d x), h0 = mlp_base output 0 before trunc_exp, x = the normalised hash-input position after the
+    in-box selector (outside the box x = 0, and the normal is the gradient at the box origin).  Takes the sample keywords
+    of field_forward plus the `offsets` a deformed evaluation produced (canonical-space normals: the deformation
+    Jacobian is not applied).  world_space=True divides the gradient by the box extent per axis before normalising.
+    With offsets, the tables are gathered as field_forward gathers them for the same call (blended frame table / timestep
+    stack unless line_gather or per-sample blend codes).  With packed_info [R,2] and weights [n] also `ray_normals`
+    [R,3] = sum_i w_i n_i / (|sum_i w_i n_i| + 1e-10).  Not differentiable.  Returns {"normals": [n,3], ...}."""
+    keep: list = []
+    s = _lib.Samples()
+    n = _fill_samples(s, keep, origins=origins, directions=directions, ray_times=ray_times, t_starts=t_starts, t_ends=t_ends,
+                      ray_indices=ray_indices, positions=positions, sample_times=sample_times,
+                      sample_blend_codes=sample_blend_codes)
+    dev = (origins if origins is not None else positions).device
+    if sample_blend_codes is not None:
+        assert tuple(sample_blend_codes.shape) == (n, 32)
+    if n_samples_dev is not None:
+        assert n_samples_dev.dtype == torch.int64 and n_samples_dev.is_cuda and n_samples_dev.numel() == 1
+        s.n_samples_dev = _ptr(n_samples_dev); keep.append(n_samples_dev)
+    frame = None
+    if offsets is not None and not line_gather and sample_blend_codes is None:
+        frame = (P.frame_table(uniform_time, window_hash, disable_initial, soft_transition) if uniform_time is not None
+                 else P.timestep_tables(window_hash, disable_initial, soft_transition))
+    opts = make_opts(window_hash, None, offsets is not None, False, disable_initial, soft_transition)
+    cp = P.c_params(inference=frame is not None, frame=frame)
+    return _normals_launch(P, cp, opts, s, n, dev, offsets=offsets,
+                           grad_scale=_world_grad_scale(P) if world_space else (1.0, 1.0, 1.0),
+                           packed_info=packed_info, weights=weights, keep=keep)
+
+
 def _fill_samples(s, keep, *, origins=None, directions=None, ray_times=None, t_starts=None, t_ends=None, ray_indices=None,
                   positions=None, sample_times=None, sample_directions=None, sample_blend_codes=None):
     if origins is not None:
@@ -856,7 +926,8 @@ class RenderResult(dict):
         if status != 0 or n > b["capacity"]:
             raise RuntimeError(f"render_rays: the march produced more samples than the workspace holds "
                                f"(n_total {n}, capacity {b['capacity']}, status {status}); pass a larger capacity")
-        out = {k: b[k][:n] for k in ("t_starts", "t_ends", "ray_indices", "sigma", "rgb", "offsets", "weights") if b.get(k) is not None}
+        out = {k: b[k][:n] for k in ("t_starts", "t_ends", "ray_indices", "sigma", "rgb", "offsets", "weights", "normals")
+               if b.get(k) is not None}
         out["weights"] = out["weights"][:, None]
         return out
 
@@ -866,7 +937,8 @@ def render_rays(P: NativeParams, origins, directions, ray_times, *, window_hash=
                 near_plane: float = 0.0, near_planes=None, far_planes=None, binaries=None, aabbs=None,
                 step: float = 1e-3, cone_angle: float = 0.0, capacity: Optional[int] = None,
                 disable_initial=True, soft_transition=True, single_launch: bool = False,
-                single_traversal: bool = True, uniform_time: Optional[float] = None, line_gather: bool = False) -> RenderResult:
+                single_traversal: bool = True, uniform_time: Optional[float] = None, line_gather: bool = False,
+                want_normals: bool = False) -> RenderResult:
     """The fused inference render (nsb_render_forward): sampler -> field -> composite without a host synchronisation.
     sampler 'fixed' (n_per_ray steps from the box entry: ONE launch) or 'occupancy' (nerfacc march of `binaries`
     [levels,res,res,res] within per-ray near_planes / far_planes: the cooperative march launch + one fused launch;
@@ -875,7 +947,9 @@ def render_rays(P: NativeParams, origins, directions, ray_times, *, window_hash=
     depth, deformation, num_samples_per_ray, packed_info); `.packed()` gives the per-sample arrays (one sync).
     capacity: per-sample workspace size; default = an upper bound of the march (rays x ceil(largest diagonal / step) + 2).
     The field gathers member-blended tables (frame_table for a uniform_time, timestep_tables otherwise) unless
-    line_gather=True forces the per-sample blend of the 128 B table lines."""
+    line_gather=True forces the per-sample blend of the 128 B table lines.
+    want_normals=True adds `normals` [R,3]: the world-space surface normals of the call's own packed samples (field_normals
+    on the same tables), composited with the render weights and normalised; still without a host synchronisation."""
     lib = _lib.load()
     origins, directions = _f32c(origins).reshape(-1, 3), _f32c(directions).reshape(-1, 3)
     ray_times = None if ray_times is None else _f32c(ray_times).reshape(-1)
@@ -932,6 +1006,8 @@ def render_rays(P: NativeParams, origins, directions, ray_times, *, window_hash=
     out["_keep"] = keep
     out["num_samples_per_ray"] = info[:, 1]
     if R == 0:
+        if want_normals:
+            out["normals"] = torch.empty((0, 3), dtype=_F32, device=dev)
         return out
     opts = make_opts(window_hash, window_deform, use_deformation, True, disable_initial, soft_transition)
     frame = None
@@ -943,6 +1019,16 @@ def render_rays(P: NativeParams, origins, directions, ray_times, *, window_hash=
             frame = P.timestep_tables(window_hash, disable_initial, soft_transition)
     cp = P.c_params(inference=True, frame=frame)
     _lib.check(lib.nsb_render_forward(C.byref(cp), C.byref(opts), C.byref(a), _stream()), "nsb_render_forward")
+    if want_normals:
+        # the pass reads the packed samples the render left in `buf`; their count stays on the device (header n_total)
+        s = _lib.Samples()
+        s.n_samples, s.n_samples_dev = cap, _ptr(ws[2:3])
+        s.origins, s.directions, s.ray_times = _ptr(origins), _ptr(directions), _ptr(ray_times)
+        s.t_starts, s.t_ends, s.ray_indices = _ptr(buf["t_starts"]), _ptr(buf["t_ends"]), _ptr(buf["ray_indices"])
+        nrm = _normals_launch(P, cp, opts, s, cap, dev, offsets=buf["offsets"], grad_scale=_world_grad_scale(P),
+                              packed_info=info, weights=buf["weights"])
+        buf["normals"] = nrm["normals"]
+        out["normals"] = nrm["ray_normals"]
     return out
 
 

@@ -62,8 +62,9 @@ def _xavier_flat(shapes, gen):
 
 class NeRSembleNeRFactoField(nn.Module):
     """Constructor keeps the reference's keyword surface (nersemble_nerfacto_field.py:32-62); options the
-    NeRSemble recipe never enables (transient / semantics / normals / appearance embedding / scene contraction /
-    SH directions) are rejected instead of silently ignored."""
+    NeRSemble recipe never enables (transient / semantics / predicted normals / appearance embedding / scene
+    contraction / SH directions) are rejected instead of silently ignored.  Analytic normals (forward(...,
+    compute_normals=True), get_normals) are supported."""
 
     def __init__(self, aabb: Tensor, num_images: int, num_layers: int = 2, hidden_dim: int = 64, geo_feat_dim: int = 15,
                  num_levels: int = 16, max_res: int = 2048, log2_hashmap_size: int = 19, num_layers_color: int = 3,
@@ -105,6 +106,7 @@ class NeRSembleNeRFactoField(nn.Module):
         self.mlp_loss_scale = 128.0      # the backward's fp16 MLP deltas are scaled by this and the gradients divided back
         self._native = None
         self._native_version = None
+        self._last_samples = None        # (positions, time_codes, window) of the last density evaluation: get_normals()
 
     # ---- parameter views
     def base_weights(self):
@@ -136,6 +138,7 @@ class NeRSembleNeRFactoField(nn.Module):
     def density_fn(self, positions: Tensor, times: Optional[Tensor] = None, window_hash_encodings: Optional[float] = None,
                    time_codes: Optional[Tensor] = None) -> Tensor:
         """nersemble_nerfacto_field.py:228-248."""
+        self._last_samples = (positions.detach(), None if time_codes is None else time_codes.detach(), window_hash_encodings)
         if _needs_grad(positions, time_codes, *self._grad_params()):
             sigma, _ = _FieldFunction.apply(self, positions, None, time_codes, window_hash_encodings, False,
                                             *self._grad_params())
@@ -155,18 +158,35 @@ class NeRSembleNeRFactoField(nn.Module):
 
     def forward(self, ray_samples: RaySamples, compute_normals: bool = False,
                 window_hash_encodings: Optional[float] = None) -> Dict[FieldHeadNames, Tensor]:
-        """nersemble_nerfacto_field.py:385-402."""
-        if compute_normals:
-            raise NotImplementedError("compute_normals")
+        """nersemble_nerfacto_field.py:385-402.  compute_normals adds FieldHeadNames.NORMALS [n,3] (get_normals; with or
+        without autograd, and not differentiable); RGB and DENSITY are the same either way."""
         if ray_samples.camera_indices is None:
             raise AttributeError("Camera indices are not provided.")
         tc = ray_samples.metadata["time_codes"]
         pos = ray_samples.frustums.get_positions()
+        self._last_samples = (pos.detach(), None if tc is None else tc.detach(), window_hash_encodings)
         if _needs_grad(pos, tc, *self._grad_params()):
             sigma, rgb = _FieldFunction.apply(self, pos, ray_samples.frustums.directions, tc, window_hash_encodings, True,
                                               *self._grad_params())
-            return {FieldHeadNames.RGB: rgb, FieldHeadNames.DENSITY: sigma[:, None]}
-        out = ops.field_forward(self._native_params(), window_hash=window_hash_encodings, use_deformation=False,
-                                positions=pos, sample_directions=ray_samples.frustums.directions, sample_blend_codes=tc,
-                                want=("sigma", "rgb"), **self._opts())
-        return {FieldHeadNames.RGB: out["rgb"], FieldHeadNames.DENSITY: out["sigma"][:, None]}
+            outputs = {FieldHeadNames.RGB: rgb, FieldHeadNames.DENSITY: sigma[:, None]}
+        else:
+            out = ops.field_forward(self._native_params(), window_hash=window_hash_encodings, use_deformation=False,
+                                    positions=pos, sample_directions=ray_samples.frustums.directions, sample_blend_codes=tc,
+                                    want=("sigma", "rgb"), **self._opts())
+            outputs = {FieldHeadNames.RGB: out["rgb"], FieldHeadNames.DENSITY: out["sigma"][:, None]}
+        if compute_normals:
+            outputs[FieldHeadNames.NORMALS] = self.get_normals()
+        return outputs
+
+    def get_normals(self) -> Tensor:
+        """nerfstudio Field.get_normals: -normalize(d h0 / d x) [n,3] for the samples of the last get_density / forward /
+        density_fn call; h0 = mlp_base output 0 before trunc_exp, x = the normalised position after the in-box selector
+        (nersemble_nerfacto_field.py:257-287).  Not differentiable (the reference takes the gradient without
+        create_graph)."""
+        if self._last_samples is None:
+            raise RuntimeError("get_normals: no density has been evaluated yet")
+        positions, time_codes, window = self._last_samples
+        with torch.no_grad():
+            out = ops.field_normals(self._native_params(), window_hash=window, positions=positions,
+                                    sample_blend_codes=time_codes, **self._opts())
+        return out["normals"]

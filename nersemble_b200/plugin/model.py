@@ -200,6 +200,8 @@ class NeRSembleNGPModel(Model):
                                            # the table one streaming pass over the hash tables)
         self.prepass_reuse = True        # ... and the pre-pass's blended features / corner values are packed with the kept
                                          # samples, so the differentiable forward does not gather the tables a second time
+        self.render_normals = False      # get_outputs / get_outputs_for_camera_ray_bundle also return "normals": world-space
+                                         # surface normals composited with the render weights (unit vectors, [R,3] / [H,W,3])
 
     def populate_modules(self):
         """models/nersemble_instant_ngp.py:81-179 (+ BaseModel.populate_modules, base.py:38-47)."""
@@ -339,7 +341,20 @@ class NeRSembleNGPModel(Model):
                                use_deformation=cfg.use_deformation_field, training=self.training, sampler="occupancy",
                                near_planes=near_planes, far_planes=far_planes, binaries=og.binaries, aabbs=og.aabbs,
                                step=cfg.render_step_size, cone_angle=cfg.cone_angle, uniform_time=uniform_time,
-                               line_gather=not self.frame_tables, **self._blend_opts())
+                               line_gather=not self.frame_tables, want_normals=self.render_normals, **self._blend_opts())
+
+    @torch.no_grad()
+    def _packed_normals(self, ray_bundle: RayBundle, ray_times, starts, ends, ray_indices, packed_info, weights, offsets,
+                        line_gather: bool) -> Tensor:
+        """Rendered normals [R,3] of packed samples the field already evaluated (the non-fused get_outputs paths):
+        world-space per-sample normals, composited with the render weights and normalised (ops.field_normals)."""
+        wh, _ = self._windows()
+        out = ops.field_normals(self.native_params(), window_hash=wh, offsets=offsets,
+                                origins=ray_bundle.origins.reshape(-1, 3), directions=ray_bundle.directions.reshape(-1, 3),
+                                ray_times=ray_times, t_starts=starts, t_ends=ends, ray_indices=ray_indices,
+                                line_gather=line_gather, world_space=True, packed_info=packed_info, weights=weights,
+                                **self._blend_opts())
+        return out["ray_normals"]
 
     @torch.no_grad()
     def _sample_packed(self, ray_bundle: RayBundle, jitter: Optional[Tensor], want_payload: bool = False):
@@ -402,7 +417,7 @@ class NeRSembleNGPModel(Model):
         for i in range(0, h * w, n):
             rb = camera_ray_bundle.get_row_major_sliced_ray_bundle(i, i + n)
             res = self._fused_render(rb, uniform_time)
-            for name in ("rgb", "accumulation", "depth", "num_samples_per_ray", "deformation"):
+            for name in ("rgb", "accumulation", "depth", "num_samples_per_ray", "deformation", "normals"):
                 if name in res:
                     lists.setdefault(name, []).append(res[name])
         return {k: torch.cat(v).view(h, w, -1) for k, v in lists.items()}
@@ -435,6 +450,8 @@ class NeRSembleNGPModel(Model):
                 if cfg.use_deformation_field:
                     ray_samples.frustums.set_offsets(pk["offsets"])
                     outputs["deformation"] = res["deformation"]
+                if self.render_normals:
+                    outputs["normals"] = res["normals"]
                 return outputs
             # no sample at all: the reference inserts one fake sample (nersemble_volumetric_sampler.py:110-114) -> general path
         if self.use_fused_sampler and self.scene_aabb.is_cuda:
@@ -473,6 +490,9 @@ class NeRSembleNGPModel(Model):
             if cfg.use_deformation_field:
                 outputs["deformation"] = res[4]
                 ray_samples.frustums.set_offsets(res[5])
+            if self.render_normals:     # the training forward gathers the table lines
+                outputs["normals"] = self._packed_normals(ray_bundle, ray_times, starts, ends, ray_indices, packed_info,
+                                                          weights, res[5] if cfg.use_deformation_field else None, True)
             return outputs
         out = ops.render_packed(self.native_params(), ray_bundle.origins, ray_bundle.directions, ray_times, starts, ends,
                                 ray_indices, packed_info, window_hash=wh, window_deform=wd,
@@ -486,6 +506,10 @@ class NeRSembleNGPModel(Model):
         }
         if cfg.use_deformation_field:
             outputs["deformation"] = out["deformation"]
+        if self.render_normals:
+            outputs["normals"] = self._packed_normals(ray_bundle, ray_times, starts, ends, ray_indices, packed_info,
+                                                      out["weights"], out["offsets"] if cfg.use_deformation_field else None,
+                                                      False)
         return outputs
 
     def update_to_step(self, step: int) -> None:

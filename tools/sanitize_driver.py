@@ -1,7 +1,7 @@
 """Small end-to-end exercise of every libnsb kernel, sized for compute-sanitizer (tools/sanitize.sh):
 fixed + occupancy march, visibility mask, fused field forward (inference and training instantiations, ragged last tile,
 several tiles per CTA so the mbarrier ring / tile counters wrap), composite fwd/bwd, losses, field / deformation
-backward, rank-1 expand + fused Adam, occupancy update, component kernels."""
+backward, rank-1 expand + fused Adam, occupancy update, component kernels, surface normals."""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
@@ -23,6 +23,10 @@ out2 = ops.render_packed(P, o, d, t, ts[:-37], te[:-37], ri[:-37],
                          window_hash=1.5, window_deform=3.3, training=False)                 # ragged last tile
 x = torch.rand((500, 3), device=dev); codes = torch.randn((500, 32), device=dev) * 0.2
 ops.hash_blend_forward(P, x, codes, window_hash=20.25)
+ops.field_normals(P, window_hash=20.25, positions=P.aabb[0].to(dev) + x * (P.aabb[1] - P.aabb[0]).to(dev), sample_blend_codes=codes)
+for lg in (False, True):        # normals of the render's packed samples: timestep stack and line gather, per-ray composite
+    ops.render_rays(P, o, d, t, window_hash=32.0, window_deform=7.0, sampler="fixed", n_per_ray=100, near_plane=bench.NEAR,
+                    step=bench.STEP, line_gather=lg, want_normals=True)
 ops.field_forward(P, window_hash=32.0, window_deform=7.0, positions=P.aabb[0].to(dev) + x * (P.aabb[1] - P.aabb[0]).to(dev),
                   sample_times=torch.rand(500, device=dev), want=("sigma",))
 # plugin model: occupancy march + pre-pass + training step + occupancy update
