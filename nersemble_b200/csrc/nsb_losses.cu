@@ -7,7 +7,8 @@
 //   losses_fwd_kernel   warp per ray: one pass over the ray's samples with shuffle scans; partial sums and counts
 //                       go to 16 double accumulators (atomicAdd, 13 per ray) -> losses_finalize_kernel -> 6 values
 //   losses_bwd_kernel   warp per ray: d rgb / d acc / d depth per ray and d weights per sample (prefix AND suffix sums of
-//                       the ray: totals first, then one more pass), scaled by the upstream gradient of each loss value
+//                       the ray: a reverse pass for the suffixes between two forward passes), scaled by the upstream
+//                       gradient of each loss value
 // Formulas (S = samples, R = rays; masks are 0/1; every mean divides by max(count, 1) except the rgb loss, which keeps
 // the reference's 0/0 = nan for an empty mask):
 //   rgb    mean over masked rays and 3 channels of (image - rgb)^2                 mask = alpha > alpha_mask_threshold
@@ -29,6 +30,22 @@ __device__ __forceinline__ float lw_incl_scan(float v, int lane) {
         if (lane >= o) v += t;
     }
     return v;
+}
+// exclusive scans: the sum over the lanes below (prefix) or above (suffix) this one
+__device__ __forceinline__ float lw_excl_scan(float v, int lane) {
+    float x = __shfl_up_sync(0xffffffffu, v, 1);
+    if (lane == 0) x = 0.f;
+    return lw_incl_scan(x, lane);
+}
+__device__ __forceinline__ float lw_excl_suffix(float v, int lane) {
+    float x = __shfl_down_sync(0xffffffffu, v, 1);
+    if (lane == 31) x = 0.f;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const float t = __shfl_down_sync(0xffffffffu, x, o);
+        if (lane + o < 32) x += t;
+    }
+    return x;
 }
 __device__ __forceinline__ float lw_sum(float v) {
 #pragma unroll
@@ -156,24 +173,51 @@ __global__ void __launch_bounds__(256) losses_bwd_kernel(const __grid_constant__
     if (cnt == 0) return;
     const float ce = g[2] * c[2], cn = g[3] * c[3], cd = g[5] * c[5];
     const bool want_near = depth_terms && tgt > 0.f && a.lambda_near > 0.f, want_empty = depth_terms && tgt > 0.f && a.lambda_empty > 0.f;
-    // pass 1: totals of w, w*m and of the near residuals r_i = (A_i - Phi_i) * near_i
-    float Wt = 0.f, WMt = 0.f, Rt = 0.f, cw = 0.f;
-    for (int64_t b = 0; b < cnt; b += 32) {
-        const int64_t i = b + lane;
-        const bool ok = i < cnt;
-        const int64_t s = start + (ok ? i : 0);
-        const float ts = ok ? a.t_starts[s] : 0.f, te = ok ? a.t_ends[s] : 0.f;
-        const float w = ok ? a.weights[s] : 0.f;
-        const float m = (ts + te) * 0.5f;
-        const float iw = lw_incl_scan(w, lane);
-        if (ok && want_near && tgt - a.eps_depth <= m && m <= tgt + a.eps_depth) Rt += (cw + iw) - normal_cdf(m - tgt, scale);
-        Wt += w; WMt += w * m;
-        cw += __shfl_sync(0xffffffffu, iw, 31);
+    // Every sum over earlier or later samples is its own scan (exclusive prefix front to back, suffix back to front), never
+    // a difference of a total and a prefix: where the true sum is 0 (e.g. no near sample behind k) it then is exactly 0.
+    // The samples' partial gradients are parked in their own d_weights slots between the passes (same thread).
+    // pass 1, front to back (near loss only): the near residuals r_i = (A_i - Phi_i) * near_i, A = inclusive scan of w
+    if (want_near) {
+        float cw = 0.f;
+        for (int64_t b = 0; b < cnt; b += 32) {
+            const int64_t i = b + lane;
+            const bool ok = i < cnt;
+            const int64_t s = start + (ok ? i : 0);
+            const float ts = ok ? a.t_starts[s] : 0.f, te = ok ? a.t_ends[s] : 0.f;
+            const float w = ok ? a.weights[s] : 0.f;
+            const float m = (ts + te) * 0.5f;
+            const float A = cw + lw_incl_scan(w, lane);
+            cw = __shfl_sync(0xffffffffu, A, 31);
+            if (ok) a.d_weights[s] = (tgt - a.eps_depth <= m && m <= tgt + a.eps_depth) ? A - normal_cdf(m - tgt, scale) : 0.f;
+        }
     }
-    Wt = lw_sum(Wt); WMt = lw_sum(WMt); Rt = lw_sum(Rt);
-    // pass 2: gradients
-    cw = 0.f;
-    float cwm = 0.f, cr = 0.f;
+    // pass 2, back to front: near  cn * sum_{i >= k} r_i   (A_i depends on w_k for all i >= k)
+    //                        dist  cd * 2 * sum_{i > k} w_i (m_i - m_k)
+    if (want_near || sel) {
+        float cr = 0.f, cw = 0.f, cwm = 0.f;   // suffix sums of the later chunks
+        for (int64_t b = ((cnt - 1) >> 5) << 5; b >= 0; b -= 32) {
+            const int64_t i = b + lane;
+            const bool ok = i < cnt;
+            const int64_t s = start + (ok ? i : 0);
+            const float ts = ok ? a.t_starts[s] : 0.f, te = ok ? a.t_ends[s] : 0.f;
+            const float w = ok ? a.weights[s] : 0.f;
+            const float m = (ts + te) * 0.5f;
+            const float r = (ok && want_near) ? a.d_weights[s] : 0.f;
+            const float Ri = cr + (lw_excl_suffix(r, lane) + r);
+            const float Wx = cw + lw_excl_suffix(w, lane), WMx = cwm + lw_excl_suffix(w * m, lane);
+            cr = __shfl_sync(0xffffffffu, Ri, 0);
+            cw = __shfl_sync(0xffffffffu, Wx + w, 0);
+            cwm = __shfl_sync(0xffffffffu, WMx + w * m, 0);
+            if (ok) {
+                float dw = 0.f;
+                if (want_near) dw += cn * Ri;
+                if (sel) dw += cd * (2.0f * (WMx - m * Wx));
+                a.d_weights[s] = dw;
+            }
+        }
+    }
+    // pass 3, front to back: empty  ce * w;  dist  cd * (2/3 dt w + 2 sum_{i < k} w_i (m_k - m_i))
+    float cw = 0.f, cwm = 0.f;   // prefix sums of the earlier chunks
     for (int64_t b = 0; b < cnt; b += 32) {
         const int64_t i = b + lane;
         const bool ok = i < cnt;
@@ -181,24 +225,15 @@ __global__ void __launch_bounds__(256) losses_bwd_kernel(const __grid_constant__
         const float ts = ok ? a.t_starts[s] : 0.f, te = ok ? a.t_ends[s] : 0.f;
         const float w = ok ? a.weights[s] : 0.f;
         const float m = (ts + te) * 0.5f;
-        const float iw = lw_incl_scan(w, lane), iwm = lw_incl_scan(w * m, lane);
-        const float A = cw + iw, WMi = cwm + iwm;
-        float r = 0.f;
-        if (ok && want_near && tgt - a.eps_depth <= m && m <= tgt + a.eps_depth) r = A - normal_cdf(m - tgt, scale);
-        const float ir = lw_incl_scan(r, lane);
+        const float Wpre = cw + lw_excl_scan(w, lane), WMpre = cwm + lw_excl_scan(w * m, lane);
+        cw = __shfl_sync(0xffffffffu, Wpre + w, 31);
+        cwm = __shfl_sync(0xffffffffu, WMpre + w * m, 31);
         if (ok) {
-            float dw = 0.f;
+            float dw = (want_near || sel) ? a.d_weights[s] : 0.f;
             if (want_empty && m < tgt - a.eps_depth) dw += ce * w;
-            if (want_near) dw += cn * (Rt - (cr + ir - r));                  // sum_{i >= k} r_i: A_i depends on w_k for all i >= k
-            if (sel) {
-                const float Wpre = A - w, WMpre = WMi - w * m;
-                dw += cd * ((2.0f / 3.0f) * (te - ts) * w + 2.0f * (m * Wpre - WMpre) + 2.0f * ((WMt - WMi) - m * (Wt - A)));
-            }
+            if (sel) dw += cd * ((2.0f / 3.0f) * (te - ts) * w + 2.0f * (m * Wpre - WMpre));
             a.d_weights[s] = dw;
         }
-        cw += __shfl_sync(0xffffffffu, iw, 31);
-        cwm += __shfl_sync(0xffffffffu, iwm, 31);
-        cr += __shfl_sync(0xffffffffu, ir, 31);
     }
 }
 

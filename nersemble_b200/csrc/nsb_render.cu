@@ -102,13 +102,27 @@ __global__ void __launch_bounds__(256) composite_kernel(const __grid_constant__ 
 }
 
 // ---------------------------------------------------------------------------------------------
-// compositing backward (training mode): one warp per ray, two passes over the ray's samples.
+// compositing backward (training mode): one warp per ray, three passes over the ray's samples.
 //   w_i = T_i a_i, T_i = exp(-sum_{j<i} sd_j), a_i = 1-exp(-sd_i), sd = sigma*dt
 //   dL/dsd_i = G_i T_i (1-a_i) - sum_{j>i} G_j w_j,  G_i = dL/dw_i (all consumers of w_i)
+// The suffix sum_{j>i} G_j w_j is a reverse scan (last chunk first), not total - inclusive prefix: behind an opaque
+// surface every later G_j w_j is exactly 0, and so is the suffix, where the subtraction leaves ~eps * |total| of noise.
 // ---------------------------------------------------------------------------------------------
 struct CompBwdArgs {
     nsb_composite_bwd_args a;
 };
+
+// exclusive reverse scan within the warp: sum of v over the lanes above this one
+__device__ __forceinline__ float warp_excl_suffix(float v, int lane) {
+    float x = __shfl_down_sync(0xffffffffu, v, 1);
+    if (lane == 31) x = 0.f;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const float t = __shfl_down_sync(0xffffffffu, x, o);
+        if (lane + o < 32) x += t;
+    }
+    return x;
+}
 
 __global__ void __launch_bounds__(256) composite_bwd_kernel(const __grid_constant__ CompBwdArgs C) {
     const nsb_composite_bwd_args &a = C.a;
@@ -143,28 +157,9 @@ __global__ void __launch_bounds__(256) composite_bwd_kernel(const __grid_constan
         if (!(draw >= lo && draw <= hi)) gdep = 0.f;
     }
     const float gbg = -(gr + gg + gb);     // white background: rgb + (1 - acc)
-    // pass 2a: total = sum_j G_j w_j
-    float total = 0.f;
+    // pass 2, front to back: the per-sample terms.  Each sample's G T e, G w, w and dt are parked in its own output slots
+    // (d_sigma, d_rgb[0..2]); pass 3 reads them back in the same thread, so no other memory is needed.
     carry = 0.f;
-    for (int64_t b = 0; b < cnt; b += 32) {
-        const int64_t i = b + lane;
-        const bool ok = i < cnt;
-        const int64_t s = start + (ok ? i : 0);
-        const float ts = ok ? a.t_starts[s] : 0.f, te = ok ? a.t_ends[s] : 0.f;
-        const float sd = ok ? a.sigma[s] * (te - ts) : 0.f;
-        const float incl = warp_incl_scan(sd, lane);
-        const float w = ok ? expf(-(carry + (incl - sd))) * (1.0f - expf(-sd)) : 0.f;
-        carry += __shfl_sync(0xffffffffu, incl, 31);
-        if (ok) {
-            const float G = (a.d_weights ? a.d_weights[s] : 0.f) + gr * a.rgb[3 * s] + gg * a.rgb[3 * s + 1] +
-                            gb * a.rgb[3 * s + 2] + gbg + gacc + gdep * (((ts + te) / 2.0f) - draw) * inv;
-            total += G * w;
-        }
-    }
-    total = warp_sum(total);
-    // pass 2b: gradients
-    carry = 0.f;
-    float pcarry = 0.f;
     for (int64_t b = 0; b < cnt; b += 32) {
         const int64_t i = b + lane;
         const bool ok = i < cnt;
@@ -177,16 +172,25 @@ __global__ void __launch_bounds__(256) composite_bwd_kernel(const __grid_constan
         const float e = expf(-sd);
         const float w = ok ? T * (1.0f - e) : 0.f;
         carry += __shfl_sync(0xffffffffu, incl, 31);
-        float G = 0.f;
-        if (ok)
-            G = (a.d_weights ? a.d_weights[s] : 0.f) + gr * a.rgb[3 * s] + gg * a.rgb[3 * s + 1] + gb * a.rgb[3 * s + 2] +
-                gbg + gacc + gdep * (((ts + te) / 2.0f) - draw) * inv;
-        const float gw = G * w;
-        const float pin = warp_incl_scan(gw, lane);          // inclusive prefix of G_j w_j
-        const float suffix = total - (pcarry + pin);          // sum_{j>i} G_j w_j
-        pcarry += __shfl_sync(0xffffffffu, pin, 31);
         if (ok) {
-            a.d_sigma[s] = (G * T * e - suffix) * dt;
+            const float G = (a.d_weights ? a.d_weights[s] : 0.f) + gr * a.rgb[3 * s] + gg * a.rgb[3 * s + 1] +
+                            gb * a.rgb[3 * s + 2] + gbg + gacc + gdep * (((ts + te) / 2.0f) - draw) * inv;
+            a.d_sigma[s] = G * T * e;
+            a.d_rgb[3 * s] = G * w; a.d_rgb[3 * s + 1] = w; a.d_rgb[3 * s + 2] = dt;
+        }
+    }
+    // pass 3, back to front: suffix = sum_{j>i} G_j w_j as a reverse scan with a carried suffix of the later chunks
+    float scarry = 0.f;
+    for (int64_t b = ((cnt - 1) >> 5) << 5; b >= 0; b -= 32) {
+        const int64_t i = b + lane;
+        const bool ok = i < cnt;
+        const int64_t s = start + (ok ? i : 0);
+        const float gte = ok ? a.d_sigma[s] : 0.f, gw = ok ? a.d_rgb[3 * s] : 0.f;
+        const float w = ok ? a.d_rgb[3 * s + 1] : 0.f, dt = ok ? a.d_rgb[3 * s + 2] : 0.f;
+        const float suffix = scarry + warp_excl_suffix(gw, lane);
+        scarry = __shfl_sync(0xffffffffu, suffix + gw, 0);
+        if (ok) {
+            a.d_sigma[s] = (gte - suffix) * dt;
             a.d_rgb[3 * s] = gr * w; a.d_rgb[3 * s + 1] = gg * w; a.d_rgb[3 * s + 2] = gb * w;
         }
     }
