@@ -365,7 +365,7 @@ __global__ void __launch_bounds__(kLaunchBoundWS, 1) field_kernel_ws_given(const
 constexpr int kFrameGatherWarps = NSB_FRAME_GATHER_WARPS;   // frame-table gather: how many of the gather warps do work
 constexpr int kTcStages = 4, kTcBlocksPerTile = 14;
 #ifdef NSB_TC_PROF
-constexpr int kTcProfPhases = 9;     // tools/tc_prof.py names them
+constexpr int kTcProfPhases = 10;    // tools/tc_prof.py names them
 __device__ unsigned long long g_tc_prof[kTcProfPhases], g_tc_prof_k[8];
 #define KPROF(i) if (threadIdx.x == 0 && blockIdx.x == 3) g_tc_prof_k[i] = (unsigned long long)clock64();
 #else
@@ -379,11 +379,18 @@ constexpr size_t kTcPackedBytes = 12 * 16384 + 2 * 2048;
 // `tid >> 5`: there the broadcast moves their gather-role register allocation and adds spills in the sample loop.
 __device__ __forceinline__ int tc_warp_index(int tid) { return __shfl_sync(0xffffffffu, tid >> 5, 0); }
 
+// Code-bias rows deform_code_bias[t][0|1][128] (fp32, 1 KB per timestep) staged in shared memory for the epilogues of
+// layers 0 and 4 of the frame-table kernels.  Up to kTcCodeBiasRows timesteps are staged; a larger table is read from
+// global memory (tc_code_bias_rows).  The rows sit over blend_b / cv_stage, which the frame gather role never touches;
+// the launch sizes the dynamic shared memory from T.
+constexpr int kTcCodeBiasRows = 32;
+constexpr int kTcBiasFloats = 4 * 128 + 8;      // sm.bias: the biases of layers 1, 2, 3, 5, then the heads (v 0..2, r 3..5)
+
 struct alignas(1024) SmemTC {
     uint8_t wring[kTcStages][16384];        // weight blocks [128 n x 64 k] (heads: [16 x 64]) in core-matrix order
-    uint8_t a_enc[16384];                   // posenc A operand [128 rows x 64 k] (the hidden layers' A stays in registers)
+    uint8_t a_enc[12288];                   // posenc A operand [128 rows x 48 k] (the hidden layers' A stays in registers)
     uint4 field_w[kFieldPackedU4];
-    alignas(16) float bias[kBiasFloats];
+    alignas(16) float bias[kTcBiasFloats];  // layers 0 and 4 take their bias from the code-bias rows
     alignas(16) float heads[2][64][8];      // deformation head outputs (v 0..2, r 3..5) of each warpgroup's 64 rows
     uint64_t full[kTcStages];
     uint64_t xs_full[2], feat_full[2];
@@ -395,19 +402,48 @@ struct alignas(1024) SmemTC {
     alignas(16) float xs[2][NSB_TILE][4];
     alignas(16) __half feat[2][NSB_TILE * kFeatStride];
     alignas(16) float dirsel[2][NSB_TILE][4];
-    uint2 blend_b[kGatherWarps][4 * 32];
+    uint2 blend_b[kGatherWarps][4 * 32];    // per-sample blend only
     uint4 cv_stage[kGatherWarps][1];        // SAVE is never instantiated with the tc role; the gather include names it
 };
-static_assert(sizeof(SmemTC) <= 227 * 1024, "shared memory plan");
+// byte offset of the staged code-bias rows in dynamic shared memory (a multiple of 128: the swizzle of NSB_TC_SETUP
+// permutes 32-byte chunks inside 128-byte lines), and the dynamic shared memory of a launch
+template <bool FRAME>
+__host__ __device__ constexpr size_t tc_code_bias_offset() {
+    return (FRAME ? offsetof(SmemTC, blend_b) + 127 : offsetof(SmemTC, cv_stage) + sizeof(SmemTC::cv_stage) + 127) / 128 * 128;
+}
+template <bool FRAME>
+__host__ __device__ constexpr size_t tc_smem_bytes(int staged_rows) { return tc_code_bias_offset<FRAME>() + (size_t)staged_rows * 1024; }
+static_assert(tc_code_bias_offset<true>() % 128 == 0 && tc_code_bias_offset<false>() % 128 == 0, "code-bias swizzle");
+static_assert(tc_smem_bytes<false>(kTcCodeBiasRows) <= 227 * 1024, "shared memory plan");
+// Frame-table kernels: with every T <= kTcCodeBiasRows staged, the kernel (+ 1 KB reserved per CTA) still fits H100's
+// 164 KB shared-memory carveout step, which leaves the gather role ~92 KB of L1.
+static_assert(tc_smem_bytes<true>(kTcCodeBiasRows) + 1024 <= 164 * 1024, "frame-table kernels: 164 KB carveout step");
 static_assert(kTensorWarps == 8, "the wgmma tensor role runs two warpgroups of 64 rows");
+// timesteps whose code-bias rows a tc launch stages in shared memory: all of them, or none (global fallback).  The
+// per-sample blend kernels (!FRAME) are bound by their gather role and read the global table.
+template <bool FRAME>
+__host__ __device__ __forceinline__ int tc_code_bias_rows(int n_timesteps) {
+    return FRAME && n_timesteps <= kTcCodeBiasRows ? n_timesteps : 0;
+}
 
-// setup shared by the tc kernels (textual for the same reason as the other role bodies)
+// setup shared by the tc kernels (textual for the same reason as the other role bodies).  The code-bias rows are stored
+// swizzled: the 32-byte chunk c (columns 8c .. 8c + 7) of timestep t's row moves to chunk c ^ (t & 3), so the 8 rows of
+// an epilogue load (8 timesteps at a 1 KB stride, which would all hit the same 8 banks) spread over the 4 bank groups.
 #define NSB_TC_SETUP()                                                                                              \
     {                                                                                                               \
         const uint4 *src = reinterpret_cast<const uint4 *>(A.P.field_packed);                                      \
         for (int i = tid; i < kFieldPackedU4; i += kThreadsWS) sm.field_w[i] = __ldg(src + i);                     \
-        for (int i = tid; i < kBiasFloats; i += kThreadsWS) sm.bias[i] = __ldg(A.P.deform_bias + i);               \
+        for (int i = tid; i < kTcBiasFloats; i += kThreadsWS)                                                      \
+            sm.bias[i] = __ldg(A.P.deform_bias + (i < 3 * 128 ? 128 + i : 256 + i));   /* skip layers 0, 4 */    \
         for (int i = tid; i < (int)(sizeof(sm.a_enc) / 16); i += kThreadsWS) reinterpret_cast<uint4 *>(&sm.a_enc)[i] = make_uint4(0u, 0u, 0u, 0u); \
+        {                                                                                                           \
+            float *const cb_s = reinterpret_cast<float *>(smem_raw + tc_code_bias_offset<FRAME>());                \
+            const float4 *cb_g = reinterpret_cast<const float4 *>(A.P.deform_code_bias);                           \
+            for (int i = tid; i < tc_code_bias_rows<FRAME>(A.P.n_timesteps) * 64; i += kThreadsWS) {                      \
+                const int t = i >> 6, c = (i >> 1) & 15;     /* 4 floats: row t, layer (i >> 5) & 1, chunk c */    \
+                *reinterpret_cast<float4 *>(cb_s + t * 256 + ((i >> 5) & 1) * 128 + (c ^ (t & 3)) * 8 + (i & 1) * 4) = __ldg(cb_g + i); \
+            }                                                                                                       \
+        }                                                                                                           \
         if (tid == 0) {                                                                                             \
             for (int s = 0; s < kTcStages; ++s) { mbar_init(&sm.full[s], 1); sm.ring_rel[s] = 0; }                \
             for (int b = 0; b < 2; ++b) {                                                                           \
@@ -830,12 +866,25 @@ static int launch_field_ws(const FieldArgs &A, cudaStream_t st) {
     return save ? launch_field_ws_<D, F, H, true>(A, st) : launch_field_ws_<D, F, H, false>(A, st);
 }
 
+// The tc role takes every row's code bias from the per-timestep table (staged in shared memory up to
+// kTcCodeBiasRows timesteps): calls with per-sample code bias (the component API's sample_warp_codes) run the *_ws
+// kernels (launch_field), and the fused render never sets one.
+static bool tc_args_ok(const FieldArgs &A) {
+    if (A.S.sample_code_bias || !A.P.deform_code_bias) {
+        set_error("tc kernels: the code bias must come from the per-timestep table deform_code_bias");
+        return false;
+    }
+    return true;
+}
+
 template <bool H, bool FR, bool ST>
 static int launch_field_tc_(const FieldArgs &A, cudaStream_t st) {
-    const size_t smem = sizeof(SmemTC);
+    if (!tc_args_ok(A)) return 1;
+    const size_t smem = tc_smem_bytes<FR>(tc_code_bias_rows<FR>(A.P.n_timesteps));
     static bool configured = false;
     if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(field_kernel_tc<H, FR, ST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaError_t e = cudaFuncSetAttribute(field_kernel_tc<H, FR, ST>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             (int)tc_smem_bytes<FR>(tc_code_bias_rows<FR>(kTcCodeBiasRows)));
         if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(field_kernel_tc): %s", cudaGetErrorString(e)); return 1; }
         configured = true;
     }
@@ -1022,10 +1071,12 @@ static_assert(sizeof(nsb_render_ws_header) == kRenderHdrBytes, "workspace header
 
 template <int SAMPLER, bool FR, bool ST>
 static int launch_render_tc_(const RenderKArgs &K, cudaStream_t st) {
-    const size_t smem = sizeof(SmemTC);
+    if (!tc_args_ok(K.F)) return 1;
+    const size_t smem = tc_smem_bytes<FR>(tc_code_bias_rows<FR>(K.F.P.n_timesteps));
     static bool configured = false;
     if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(render_kernel_tc<SAMPLER, FR, ST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaError_t e = cudaFuncSetAttribute(render_kernel_tc<SAMPLER, FR, ST>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             (int)tc_smem_bytes<FR>(tc_code_bias_rows<FR>(kTcCodeBiasRows)));
         if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(render_kernel_tc): %s", cudaGetErrorString(e)); return 1; }
         configured = true;
     }

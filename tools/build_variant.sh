@@ -9,5 +9,5 @@ mkdir -p $OUT
 /usr/local/cuda/bin/nvcc -O3 -std=c++17 -lineinfo -Xcompiler -fPIC -I../../include -gencode arch=compute_90a,code=sm_90a -Xptxas -v \
     $FLAGS -c nsb_field.cu -o $OUT/$NAME.field.o 2> $OUT/$NAME.ptxas.log || (cat $OUT/$NAME.ptxas.log; false)
 /usr/local/cuda/bin/nvcc -shared -gencode arch=compute_90a,code=sm_90a -o $OUT/$NAME.so $OUT/$NAME.field.o \
-    nsb_api.o nsb_render.o nsb_backward.o nsb_deform_bwd.o nsb_optim.o nsb_losses.o nsb_rays.o -lcudart
+    nsb_api.o nsb_render.o nsb_backward.o nsb_deform_bwd.o nsb_optim.o nsb_losses.o nsb_rays.o nsb_normals.o -lcudart
 python ../../tools/spill_report.py $OUT/$NAME.field.o kernel_tc

@@ -13,8 +13,9 @@ ts, te, ri, info = ops.march_fixed(o, d, P.aabb, bench.SAMPLES_PER_RAY, bench.ST
 tu = torch.full_like(t, 0.5)
 lib = _lib.load()
 lib.nsb_debug_tc_prof.argtypes = [C.c_void_p]
-names = ["feature wait + loop", "input loads", "posenc", "posenc barrier", "MMA (issue+exec+commit) wait",
-         "epilogues, layers 1-3 and 5", "heads+SE3+xs", "density / colour MLPs", "epilogues, layers 0 and 4 (code bias)"]
+names = ["feature wait + loop", "input loads", "posenc", "posenc barrier", "MMA completion (issue + wg_wait)",
+         "epilogues, layers 1-3 and 5", "heads+SE3+xs", "density / colour MLPs", "epilogues, layers 0 and 4 (code bias)",
+         "weight-ring wait (wait_blocks)"]
 tiles = (ts.numel() // 128 + 131 - 3) // 132
 for label, kw in (("per-sample blend", dict(ray_times=t)), ("frame table", dict(ray_times=tu, uniform_time=0.5)),
                   ("fused render kernel, fixed march, per-sample blend", None)):
