@@ -371,10 +371,11 @@ int nsb_occ_update(float *occs, uint8_t *binaries, int64_t n_cells, const int64_
                    int64_t n, float ema_decay, float occ_thre, void *scratch, void *stream);
 size_t nsb_occ_update_scratch_bytes(int64_t n_cells);
 
-/* ONE-LAUNCH fused inference render (SURVEY 8b `nsb_render_forward`; models/nersemble_instant_ngp.py:280-364 in eval
- * mode): sampler (fixed-stride march or nerfacc occupancy march: count -> scan -> fill) -> fused field kernel
- * (deformation MLP, hash ensemble, density / colour MLPs) -> alpha compositing + global depth clip, as phases of one
- * persistent cooperative kernel (grid = number of SMs) separated by grid-wide barriers.  The packed-sample count never
+/* Fused inference render (SURVEY 8b `nsb_render_forward`; models/nersemble_instant_ngp.py:280-364 in eval mode):
+ * sampler -> fused field kernel (deformation MLP, hash ensemble, density / colour MLPs) -> alpha compositing + global
+ * depth clip, as phases of one persistent cooperative kernel (grid = number of SMs) separated by grid-wide barriers.
+ * The fixed-stride march is a phase of that kernel; the nerfacc occupancy march (count -> scan -> fill, or one traversal
+ * into per-ray slots) is a cooperative launch of its own just before it.  The packed-sample count never
  * leaves the device, so the call is free of host synchronisation; the per-sample arrays live in a caller-provided
  * workspace of `capacity` samples (an upper bound such as n_rays * ceil(aabb diagonal / step); if the march produces
  * more, the samples beyond it are dropped and `status` in the workspace header is set to 1).
@@ -383,7 +384,8 @@ typedef struct nsb_render_args {
     int64_t n_rays;
     const float *origins, *directions; /* [n_rays][3] */
     const float *ray_times;            /* [n_rays] in [0,1] or NULL */
-    int32_t sampler;                   /* 0: fixed-stride march (n_per_ray steps from max(t_enter, near_plane)); 1: occupancy march */
+    int32_t sampler;                   /* 0: fixed-stride march (n_per_ray steps from max(t_enter, near_plane)); 1: occupancy
+                                          march; any other value is rejected */
     int32_t n_per_ray;                 /* sampler 0 */
     float near_plane;                  /* sampler 0 */
     const float *near_planes, *far_planes; /* sampler 1: [n_rays] (jitter already added) */

@@ -81,16 +81,10 @@ __device__ __forceinline__ void se3_apply(const float p[3], const float r[3], co
 // The reverse (buffer-free) edges are implied by program order: tensor warps issue D(i+2) only after
 // F(i), which waited for feat_full(i), i.e. for every gather warp to be done with tile i.
 // ===========================================================================================
-#ifndef NSB_WS_MT
-#define NSB_WS_MT 1
-#endif
-constexpr int kMT = NSB_WS_MT;                    // m-tiles (16 rows) per tensor warp
+constexpr int kMT = 1;                            // m-tiles (16 rows) per tensor warp
 constexpr int kTRows = 16 * kMT;                  // rows per tensor warp
-constexpr int kTensorWarps = NSB_TILE / kTRows;   // 8 (kMT=1) or 4 (kMT=2)
-#ifndef NSB_GATHER_WARPS
-#define NSB_GATHER_WARPS 8
-#endif
-constexpr int kGatherWarps = NSB_GATHER_WARPS;    // multiple of 4: setmaxnreg works on warpgroups
+constexpr int kTensorWarps = NSB_TILE / kTRows;   // 8
+constexpr int kGatherWarps = 8;                   // multiple of 4: setmaxnreg works on warpgroups
 constexpr int kThreadsWS = (kTensorWarps + kGatherWarps) * 32;
 // Register budget: the kernels are launched with kLaunchRegs registers per thread (the SM's 65536 over the CTA's threads,
 // in units of 8).  setmaxnreg can only move registers WITHIN the CTA's allocation (inc blocks until a dec released
@@ -100,14 +94,8 @@ constexpr int kThreadsWS = (kTensorWarps + kGatherWarps) * 32;
 // fewer registers per thread) sm_90 ptxas spills in the gather role's sample loop, and the wgmma tensor role spills below
 // 104 registers (tools/spill_report.py).
 constexpr int kLaunchRegs = (65536 / kThreadsWS) & ~7;
-#ifndef NSB_GATHER_REGS
-#define NSB_GATHER_REGS 120
-#endif
-#ifndef NSB_TENSOR_REGS
-#define NSB_TENSOR_REGS 136
-#endif
-constexpr int kGatherRegs = NSB_GATHER_REGS;
-constexpr int kTensorRegs = NSB_TENSOR_REGS;
+constexpr int kGatherRegs = 120;
+constexpr int kTensorRegs = 136;
 static_assert(kTensorWarps * 32 * kTensorRegs + kGatherWarps * 32 * kGatherRegs <= kThreadsWS * kLaunchRegs, "register pool");
 constexpr int kLaunchBoundWS = kThreadsWS;
 // Slab layout of deform_packed_tb: layers 0 and 4 without their 128 warp-code columns (those enter as the
@@ -359,10 +347,7 @@ __global__ void __launch_bounds__(kLaunchBoundWS, 1) field_kernel_ws_given(const
 // nsb_field_tensor_role_tc.inc.  The gather role is the unchanged include; only the tensor role and the shared-memory
 // plan differ.
 // ===========================================================================================
-#ifndef NSB_FRAME_GATHER_WARPS
-#define NSB_FRAME_GATHER_WARPS 8
-#endif
-constexpr int kFrameGatherWarps = NSB_FRAME_GATHER_WARPS;   // frame-table gather: how many of the gather warps do work
+constexpr int kFrameGatherWarps = 8;   // frame-table gather: how many of the gather warps do work
 constexpr int kTcStages = 4, kTcBlocksPerTile = 14;
 #ifdef NSB_TC_PROF
 constexpr int kTcProfPhases = 10;    // tools/tc_prof.py names them
@@ -506,9 +491,10 @@ __global__ void __launch_bounds__(kLaunchBoundWS, 1) field_kernel_ws_dyn(const _
 // ===========================================================================================
 // render_kernel_ws: sampler -> field -> composite in ONE launch (north star: "fused into one kernel").
 // A persistent cooperative kernel, one CTA per SM, whose phases are separated by grid-wide barriers:
-//   S  sampler.  Fixed stride: one warp per ray (march_fixed_warp).  Occupancy grid (nerfacc traverse_grids): count per ray
-//      (one thread per ray) | barrier | per-CTA chunk sums | barrier | exclusive scan -> packed_info, total | barrier |
-//      fill.  The packed sample count stays on the device (shared-memory word n_dyn): no host synchronisation.
+//   S  sampler.  Fixed stride: one warp per ray (march_fixed_warp).  Occupancy grid (nerfacc traverse_grids): the
+//      samples come from march_occ_coop_kernel (nsb_render.cu), launched just before, and the phase reads their count
+//      from the workspace header.  The packed sample count stays on the device (shared-memory word n_dyn): no host
+//      synchronisation.
 //   F  the field phase = the body of field_kernel_ws, textually (same setup / gather role / tensor role includes).
 //   C  compositing by the tensor warps (composite_ray, one warp per ray) | barrier | global depth clip.
 // Per-sample sigma / rgb / offsets cross from F to C through the caller's workspace (32 B per sample: L2-resident
@@ -547,17 +533,6 @@ __device__ __forceinline__ void grid_barrier(uint32_t *ctr, const uint32_t targe
     phase_sync();
 }
 
-__device__ __forceinline__ int64_t phase_sum_i64(int64_t v, int64_t *smem_warp /* [kTensorWarps] */, const int tid) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    phase_sync();
-    if ((tid & 31) == 0) smem_warp[tid >> 5] = v;
-    phase_sync();
-    int64_t t = 0;
-    for (int w = 0; w < kTensorWarps; ++w) t += smem_warp[w];
-    return t;
-}
-
 // Where the extra phases run.  The 64-register gather role is allocated erratically by ptxas: with the sampler phase
 // inline, or as a call ahead of the role split, it went from 1 to 37-82 spill instructions (tools/spill_report.py;
 // a spill in the sample loop costs more than everything this kernel saves).  So BOTH extra phases run on the TENSOR
@@ -565,14 +540,8 @@ __device__ __forceinline__ int64_t phase_sum_i64(int64_t v, int64_t *smem_warp /
 // on which they wait for the sampler (and the sample count in shared memory) before their first tile.
 constexpr int kPhaseThreads = kTensorWarps * 32;
 
-#ifndef NSB_RK_SAMPLER_ATTR
-#define NSB_RK_SAMPLER_ATTR __forceinline__
-#endif
-#ifndef NSB_RK_COMPOSITE_ATTR
-#define NSB_RK_COMPOSITE_ATTR __forceinline__
-#endif
-// SAMPLER: 0 fixed-stride march fused; 1 occupancy march fused (count | scan | fill); 2 samples GIVEN: a preceding
-// launch (march_occ_coop_kernel, nsb_render.cu) filled the packed arrays and left the count in the workspace header.
+// SAMPLER: 0 fixed-stride march fused; 2 samples GIVEN: a preceding launch (march_occ_coop_kernel, nsb_render.cu) filled
+// the packed arrays and left the count in the workspace header; 4 either of the two, chosen at run time by K.sampler.
 // the fixed-stride march of this CTA's rays as a real call (tensor warps, after the role split)
 __device__ __noinline__ void fixed_march_rays(const RenderKArgs &K, const int warp, const int lane) {
     const int64_t R = K.C.n_rays;
@@ -584,8 +553,7 @@ __device__ __noinline__ void fixed_march_rays(const RenderKArgs &K, const int wa
 }
 
 template <int SAMPLER, class SM = SmemWS>
-__device__ NSB_RK_SAMPLER_ATTR void render_sampler_phase(const RenderKArgs &K) {
-    constexpr bool OCC = SAMPLER == 1;
+__device__ __forceinline__ void render_sampler_phase(const RenderKArgs &K) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     SM &sm = *reinterpret_cast<SM *>(smem_raw);
     const FieldArgs &A = K.F;
@@ -613,7 +581,7 @@ __device__ NSB_RK_SAMPLER_ATTR void render_sampler_phase(const RenderKArgs &K) {
     } else if constexpr (SAMPLER == 2) {
         if (tid == 0) sm.n_dyn = min(__ldcg(&K.hdr->n_total), K.capacity);
         grid_barrier(bar, 1u * gridDim.x);          // depth_range initialised before any CTA composites
-    } else if constexpr (!OCC) {
+    } else {
         for (int64_t r = (int64_t)blockIdx.x * kTensorWarps + warp; r < R; r += (int64_t)gridDim.x * kTensorWarps) {
             const float t0 = march_fixed_t0(A.S.origins, A.S.directions, A.P.aabb, r, K.near_plane);
             march_fixed_warp(t0, r, K.n_per_ray, K.M.step, K.M.t_starts, K.M.t_ends, K.M.ray_indices, lane);
@@ -624,81 +592,18 @@ __device__ NSB_RK_SAMPLER_ATTR void render_sampler_phase(const RenderKArgs &K) {
             if (blockIdx.x == 0) K.hdr->n_total = R * K.n_per_ray;
         }
         grid_barrier(bar, 1u * gridDim.x);
-    } else {
-        // S1: samples per ray
-        for (int64_t r = (int64_t)blockIdx.x * kPhaseThreads + tid; r < R; r += (int64_t)gridDim.x * kPhaseThreads)
-            K.M.counts[r] = march_occ_ray<false, 1>(K.M, r, 0, 0);
-        grid_barrier(bar, 1u * gridDim.x);
-        // S2: exclusive scan of the counts: CTA b owns the contiguous chunk [b * chunk, (b + 1) * chunk)
-        int64_t *red = reinterpret_cast<int64_t *>(sm.ring);          // scratch: the weight ring is not live yet
-        const int64_t chunk = (R + gridDim.x - 1) / gridDim.x;
-        const int64_t r0 = min(R, (int64_t)blockIdx.x * chunk), r1 = min(R, r0 + chunk);
-        {
-            int64_t v = 0;
-            for (int64_t r = r0 + tid; r < r1; r += kPhaseThreads) v += __ldcg(K.M.counts + r);
-            const int64_t tot = phase_sum_i64(v, red, tid);
-            if (tid == 0) K.partials[blockIdx.x] = tot;
-        }
-        grid_barrier(bar, 2u * gridDim.x);
-        {
-            int64_t before = 0, total = 0;
-            for (int b = tid; b < (int)gridDim.x; b += kPhaseThreads) {
-                const int64_t p = __ldcg(K.partials + b);
-                total += p;
-                if (b < (int)blockIdx.x) before += p;
-            }
-            total = phase_sum_i64(total, red, tid);
-            before = phase_sum_i64(before, red, tid);
-            if (tid == 0) {
-                sm.n_dyn = min(total, K.capacity);
-                if (blockIdx.x == 0) { K.hdr->n_total = total; if (total > K.capacity) K.hdr->status = 1; }
-            }
-            // slabs of kPhaseThreads rays: warp scan + warp totals in shared memory + running carry
-            int64_t carry = before;
-            for (int64_t s0 = r0; s0 < r1; s0 += kPhaseThreads) {
-                const int64_t r = s0 + tid;
-                const int64_t c = r < r1 ? (int64_t)__ldcg(K.M.counts + r) : 0;
-                int64_t inc = c;
-#pragma unroll
-                for (int o = 1; o < 32; o <<= 1) {
-                    const int64_t nb = __shfl_up_sync(0xffffffffu, inc, o);
-                    if (lane >= o) inc += nb;
-                }
-                phase_sync();
-                if (lane == 31) red[warp] = inc;
-                phase_sync();
-                int64_t wbase = 0, slab = 0;
-                for (int w = 0; w < kTensorWarps; ++w) {
-                    const int64_t t = red[w];
-                    if (w < warp) wbase += t;
-                    slab += t;
-                }
-                if (r < r1) {   // beyond the caller's capacity (status = 1) rays are truncated: nothing downstream reads out of bounds
-                    const int64_t st = min(carry + wbase + inc - c, K.capacity);
-                    K.packed_info[2 * r] = st;
-                    K.packed_info[2 * r + 1] = min(c, K.capacity - st);
-                }
-                carry += slab;
-            }
-        }
-        grid_barrier(bar, 3u * gridDim.x);
-        // S3: fill (packed_info of a ray may come from another CTA: L2 reads)
-        for (int64_t r = (int64_t)blockIdx.x * kPhaseThreads + tid; r < R; r += (int64_t)gridDim.x * kPhaseThreads)
-            march_occ_ray<true, 1>(K.M, r, __ldcg(K.C.packed_info + 2 * r), K.capacity);
-        grid_barrier(bar, 4u * gridDim.x);
     }
 }
 
-template <int SAMPLER>
-__device__ NSB_RK_COMPOSITE_ATTR void render_composite_phase(const RenderKArgs &K) {
-    constexpr uint32_t kBarS = SAMPLER == 1 ? 4u : 1u;
+// the grid barriers continue the count of render_sampler_phase, which ended with barrier 1
+__device__ __forceinline__ void render_composite_phase(const RenderKArgs &K) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     uint32_t *const bar = &K.hdr->barrier;
     const int64_t R = K.C.n_rays;
-    grid_barrier(bar, (kBarS + 1u) * gridDim.x);
+    grid_barrier(bar, 2u * gridDim.x);
     for (int64_t ray = (int64_t)blockIdx.x * kTensorWarps + warp; ray < R; ray += (int64_t)gridDim.x * kTensorWarps)
         composite_ray(K.C, ray, lane);
-    grid_barrier(bar, (kBarS + 2u) * gridDim.x);
+    grid_barrier(bar, 3u * gridDim.x);
     {   // DepthRenderer('expected'): clip to the global [min, max] of the sample midpoints
         const uint32_t lo_u = __ldcg(&K.hdr->depth_range[0]), hi_u = __ldcg(&K.hdr->depth_range[1]);
         // no sample in the whole batch: the reference inserts one fake sample with t_start = t_end = 1 on ray 0
@@ -735,7 +640,7 @@ __global__ void __launch_bounds__(kLaunchBoundWS, 1) render_kernel_ws(const __gr
 #include "nsb_field_tensor_role.inc"
     }
 #undef NSB_N_SAMPLES
-    render_composite_phase<SAMPLER>(K);                                    // C
+    render_composite_phase(K);                                             // C
 }
 
 // render_kernel_ws with the deformation MLP on wgmma (nsb_field_tensor_role_tc.inc); SAMPLER 2 or 4
@@ -770,7 +675,7 @@ __global__ void __launch_bounds__(kLaunchBoundWS, 1) render_kernel_tc(const __gr
     }
 #undef NSB_N_SAMPLES
     KPROF(3)
-    render_composite_phase<SAMPLER>(K);
+    render_composite_phase(K);
     KPROF(4)
 }
 
@@ -793,10 +698,6 @@ __global__ void __launch_bounds__(256) hash_blend_kernel(const __grid_constant__
     const int64_t n_warps = (int64_t)gridDim.x * (blockDim.x >> 5);
     for (int64_t s = warp_global; s < H.n; s += n_warps) {
         const float x = H.x[3 * s + 0], y = H.x[3 * s + 1], z = H.x[3 * s + 2];
-#if NSB_GATHER_MMA
-        const BlendB Bf = make_blend_b(H.O, H.codes + s * NSB_MEMBERS, lane);
-        const float val = gather_blend_mma(H.P, x, y, z, Bf, lane);
-#else
         const int mg = lane & 7;
         float4 c = __ldg(reinterpret_cast<const float4 *>(H.codes + s * NSB_MEMBERS) + mg);
         float cw[4];
@@ -805,7 +706,6 @@ __global__ void __launch_bounds__(256) hash_blend_kernel(const __grid_constant__
         cw[2] = fmaf(c.z, H.O.cw_scale[4 * mg + 2], H.O.cw_bias[4 * mg + 2]);
         cw[3] = fmaf(c.w, H.O.cw_scale[4 * mg + 3], H.O.cw_bias[4 * mg + 3]);
         const float val = gather_blend<2>(H.P, x, y, z, cw, lane);
-#endif
         if (H.out_is_half)
             reinterpret_cast<__half *>(H.out)[s * 32 + lane] = __float2half_rn(val);
         else
@@ -827,43 +727,46 @@ static int num_sms() {
     return g_num_sms;
 }
 
-template <bool D, bool F, bool H, bool SV>
-static int launch_field_ws_(const FieldArgs &A, cudaStream_t st) {
-    const size_t smem = sizeof(SmemWS);
+constexpr size_t kRenderHdrBytes = 64, kRenderPartials = 1024;
+static_assert(sizeof(nsb_render_ws_header) == kRenderHdrBytes, "workspace header layout");
+
+// Launch of a persistent kernel (kThreadsWS threads per CTA).  The kernel's dynamic shared-memory limit is raised to
+// max_smem on its first launch.  coop_barrier != nullptr makes it a cooperative launch (the render kernels: their grid
+// barriers need every CTA resident) whose barrier counter *coop_barrier is zeroed first.
+template <auto Kernel, class Args>
+static int launch_persistent(const Args &a, size_t smem, size_t max_smem, int grid, uint32_t *coop_barrier,
+                             const char *name, cudaStream_t st) {
     static bool configured = false;
     if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(field_kernel_ws<D, F, H, SV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) {
-            set_error("cudaFuncSetAttribute(field_kernel_ws): %s", cudaGetErrorString(e));
-            return 1;
-        }
+        cudaError_t e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)max_smem);
+        if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(%s): %s", name, cudaGetErrorString(e)); return 1; }
         configured = true;
     }
-    const int64_t n_tiles = (A.S.n_samples + NSB_TILE - 1) / NSB_TILE;
-    const int grid = (int)std::min<int64_t>(n_tiles, (int64_t)num_sms());
-    field_kernel_ws<D, F, H, SV><<<grid, kThreadsWS, smem, st>>>(A);
-    return check_launch("field_kernel_ws");
-}
-// device-side sample count: instantiated for the field evaluations of the training sampler (density pre-pass; SAVE for the
-// pre-pass-reuse variant) -- each instantiation costs ~15 s of ptxas
-template <bool D, bool F, bool H, bool SV>
-static int launch_field_ws_dyn_(const FieldArgs &A, cudaStream_t st) {
-    const size_t smem = sizeof(SmemWS);
-    static bool configured = false;
-    if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(field_kernel_ws_dyn<D, F, H, SV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(field_kernel_ws_dyn): %s", cudaGetErrorString(e)); return 1; }
-        configured = true;
+    if (!coop_barrier) {
+        Kernel<<<grid, kThreadsWS, smem, st>>>(a);
+        return check_launch(name);
     }
-    const int64_t n_tiles = (A.S.n_samples + NSB_TILE - 1) / NSB_TILE;
-    const int grid = (int)std::min<int64_t>(n_tiles, (int64_t)num_sms());
-    field_kernel_ws_dyn<D, F, H, SV><<<grid, kThreadsWS, smem, st>>>(A);
-    return check_launch("field_kernel_ws_dyn");
+    if ((size_t)grid > kRenderPartials) { set_error("nsb_render_forward: more SMs than scan partials"); return 1; }
+    cudaError_t e = cudaMemsetAsync(coop_barrier, 0, sizeof(uint32_t), st);
+    if (e != cudaSuccess) { set_error("nsb_render_forward: memset: %s", cudaGetErrorString(e)); return 2; }
+    void *kargs[] = {const_cast<Args *>(&a)};
+    e = cudaLaunchCooperativeKernel(reinterpret_cast<const void *>(Kernel), dim3(grid), dim3(kThreadsWS), kargs, smem, st);
+    if (e != cudaSuccess) { set_error("%s: %s", name, cudaGetErrorString(e)); return 2; }
+    return check_launch(name);
 }
+
+// grid of the field kernels: one CTA per tile, at most one per SM
+static int field_grid(const FieldArgs &A) {
+    const int64_t n_tiles = (A.S.n_samples + NSB_TILE - 1) / NSB_TILE;
+    return (int)std::min<int64_t>(n_tiles, (int64_t)num_sms());
+}
+
 template <bool D, bool F, bool H>
 static int launch_field_ws(const FieldArgs &A, cudaStream_t st) {
     const bool save = A.out.xs || A.out.deform_acts || A.out.deform_enc || A.out.corner_vals;
-    return save ? launch_field_ws_<D, F, H, true>(A, st) : launch_field_ws_<D, F, H, false>(A, st);
+    constexpr size_t smem = sizeof(SmemWS);
+    return save ? launch_persistent<field_kernel_ws<D, F, H, true>>(A, smem, smem, field_grid(A), nullptr, "field_kernel_ws", st)
+                : launch_persistent<field_kernel_ws<D, F, H, false>>(A, smem, smem, field_grid(A), nullptr, "field_kernel_ws", st);
 }
 
 // The tc role takes every row's code bias from the per-timestep table (staged in shared memory up to
@@ -880,38 +783,14 @@ static bool tc_args_ok(const FieldArgs &A) {
 template <bool H, bool FR, bool ST>
 static int launch_field_tc_(const FieldArgs &A, cudaStream_t st) {
     if (!tc_args_ok(A)) return 1;
-    const size_t smem = tc_smem_bytes<FR>(tc_code_bias_rows<FR>(A.P.n_timesteps));
-    static bool configured = false;
-    if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(field_kernel_tc<H, FR, ST>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             (int)tc_smem_bytes<FR>(tc_code_bias_rows<FR>(kTcCodeBiasRows)));
-        if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(field_kernel_tc): %s", cudaGetErrorString(e)); return 1; }
-        configured = true;
-    }
-    const int64_t n_tiles = (A.S.n_samples + NSB_TILE - 1) / NSB_TILE;
-    const int grid = (int)std::min<int64_t>(n_tiles, (int64_t)num_sms());
-    field_kernel_tc<H, FR, ST><<<grid, kThreadsWS, smem, st>>>(A);
-    return check_launch("field_kernel_tc");
+    return launch_persistent<field_kernel_tc<H, FR, ST>>(A, tc_smem_bytes<FR>(tc_code_bias_rows<FR>(A.P.n_timesteps)),
+                                                         tc_smem_bytes<FR>(tc_code_bias_rows<FR>(kTcCodeBiasRows)),
+                                                         field_grid(A), nullptr, "field_kernel_tc", st);
 }
 template <bool H>
 static int launch_field_tc(const FieldArgs &A, cudaStream_t st) {
     if (!A.P.frame_table) return launch_field_tc_<H, false, false>(A, st);
     return A.P.frame_stride ? launch_field_tc_<H, true, true>(A, st) : launch_field_tc_<H, true, false>(A, st);
-}
-
-template <bool D>
-static int launch_field_given(const FieldArgs &A, cudaStream_t st) {
-    const size_t smem = sizeof(SmemWS);
-    static bool configured = false;
-    if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(field_kernel_ws_given<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(field_kernel_ws_given): %s", cudaGetErrorString(e)); return 1; }
-        configured = true;
-    }
-    const int64_t n_tiles = (A.S.n_samples + NSB_TILE - 1) / NSB_TILE;
-    const int grid = (int)std::min<int64_t>(n_tiles, (int64_t)num_sms());
-    field_kernel_ws_given<D><<<grid, kThreadsWS, smem, st>>>(A);
-    return check_launch("field_kernel_ws_given");
 }
 
 // The frame-table gather forms timestep * frame_stride + entry in 32 bits
@@ -921,15 +800,20 @@ static bool frame_stride_ok(const nsb_field_params *p) {
 
 template <bool D, bool F, bool H>
 static int launch_field(const FieldArgs &A, cudaStream_t st) {
+    constexpr size_t smem = sizeof(SmemWS);
     if (A.S.given_feat) {
-        if (F && H && !A.S.n_samples_dev) return launch_field_given<D>(A, st);
+        if (F && H && !A.S.n_samples_dev)
+            return launch_persistent<field_kernel_ws_given<D>>(A, smem, smem, field_grid(A), nullptr, "field_kernel_ws_given", st);
         set_error("nsb_field_forward: given_feat needs the full evaluation (rgb) and a host-side sample count");
         return 1;
     }
     if (A.S.n_samples_dev) {
-        // always the SAVE instantiation (its stores are skipped at run time when the pointers are NULL): ptxas gives its
-        // gather role 0 spill instructions, the non-SAVE density instantiation 37 (tools/spill_report.py)
-        if (F && !H) return launch_field_ws_dyn_<D, true, false, true>(A, st);
+        // device-side sample count: the density pre-pass of the training sampler (each instantiation costs ~15 s of
+        // ptxas).  Always the SAVE instantiation (its stores are skipped at run time when the pointers are NULL): ptxas
+        // gives its gather role 0 spill instructions, the non-SAVE density instantiation 37 (tools/spill_report.py)
+        if (F && !H)
+            return launch_persistent<field_kernel_ws_dyn<D, true, false, true>>(A, smem, smem, field_grid(A), nullptr,
+                                                                                "field_kernel_ws_dyn", st);
         set_error("nsb_field_forward: n_samples_dev is supported for the density evaluation (no rgb) only");
         return 1;
     }
@@ -1066,28 +950,13 @@ extern "C" int nsb_blend_tables(const nsb_field_params *params, const nsb_field_
 // nsb_render_forward: host side of render_kernel_ws
 // -------------------------------------------------------------------------------------------
 namespace nsb {
-constexpr size_t kRenderHdrBytes = 64, kRenderPartials = 1024;
-static_assert(sizeof(nsb_render_ws_header) == kRenderHdrBytes, "workspace header layout");
-
+// The render kernels run one CTA per SM, all resident: the grid barriers rely on it (the cooperative launch checks it).
 template <int SAMPLER, bool FR, bool ST>
 static int launch_render_tc_(const RenderKArgs &K, cudaStream_t st) {
     if (!tc_args_ok(K.F)) return 1;
-    const size_t smem = tc_smem_bytes<FR>(tc_code_bias_rows<FR>(K.F.P.n_timesteps));
-    static bool configured = false;
-    if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(render_kernel_tc<SAMPLER, FR, ST>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             (int)tc_smem_bytes<FR>(tc_code_bias_rows<FR>(kTcCodeBiasRows)));
-        if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(render_kernel_tc): %s", cudaGetErrorString(e)); return 1; }
-        configured = true;
-    }
-    const int grid = num_sms();
-    if ((size_t)grid > kRenderPartials) { set_error("nsb_render_forward: more SMs than scan partials"); return 1; }
-    cudaError_t e = cudaMemsetAsync(&K.hdr->barrier, 0, sizeof(uint32_t), st);
-    if (e != cudaSuccess) { set_error("nsb_render_forward: memset: %s", cudaGetErrorString(e)); return 2; }
-    void *kargs[] = {const_cast<RenderKArgs *>(&K)};
-    e = cudaLaunchCooperativeKernel(reinterpret_cast<const void *>(render_kernel_tc<SAMPLER, FR, ST>), dim3(grid), dim3(kThreadsWS), kargs, smem, st);
-    if (e != cudaSuccess) { set_error("render_kernel_tc: %s", cudaGetErrorString(e)); return 2; }
-    return check_launch("render_kernel_tc");
+    return launch_persistent<render_kernel_tc<SAMPLER, FR, ST>>(K, tc_smem_bytes<FR>(tc_code_bias_rows<FR>(K.F.P.n_timesteps)),
+                                                                tc_smem_bytes<FR>(tc_code_bias_rows<FR>(kTcCodeBiasRows)),
+                                                                num_sms(), &K.hdr->barrier, "render_kernel_tc", st);
 }
 template <int SAMPLER>
 static int launch_render_tc(const RenderKArgs &K, cudaStream_t st) {
@@ -1097,26 +966,12 @@ static int launch_render_tc(const RenderKArgs &K, cudaStream_t st) {
 
 template <bool D, int SAMPLER>
 static int launch_render(const RenderKArgs &K, cudaStream_t st) {
-    if constexpr (D && SAMPLER != 1)
+    if constexpr (D)
         if (K.F.P.deform_packed_umma)       // every instantiation is its own draw of ptxas' allocation: the fixed march
             // runs the <4> binary (run-time sampler choice, fixed march as a call), given samples the <2> binary
             return SAMPLER == 0 ? launch_render_tc<4>(K, st) : launch_render_tc<2>(K, st);
-    const size_t smem = sizeof(SmemWS);
-    static bool configured = false;
-    if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(render_kernel_ws<D, SAMPLER>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(render_kernel_ws): %s", cudaGetErrorString(e)); return 1; }
-        configured = true;
-    }
-    const int grid = num_sms();     // one CTA per SM, all resident: the grid barriers rely on it (cooperative launch checks)
-    if ((size_t)grid > kRenderPartials) { set_error("nsb_render_forward: more SMs than scan partials"); return 1; }
-    cudaError_t e = cudaMemsetAsync(&K.hdr->barrier, 0, sizeof(uint32_t), st);
-    if (e != cudaSuccess) { set_error("nsb_render_forward: memset: %s", cudaGetErrorString(e)); return 2; }
-    void *kargs[] = {const_cast<RenderKArgs *>(&K)};
-    e = cudaLaunchCooperativeKernel(reinterpret_cast<const void *>(render_kernel_ws<D, SAMPLER>), dim3(grid), dim3(kThreadsWS),
-                                    kargs, smem, st);
-    if (e != cudaSuccess) { set_error("render_kernel_ws: %s", cudaGetErrorString(e)); return 2; }
-    return check_launch("render_kernel_ws");
+    return launch_persistent<render_kernel_ws<D, SAMPLER>>(K, sizeof(SmemWS), sizeof(SmemWS), num_sms(), &K.hdr->barrier,
+                                                           "render_kernel_ws", st);
 }
 }  // namespace nsb
 
@@ -1143,12 +998,9 @@ extern "C" int nsb_render_forward(const nsb_field_params *params, const nsb_fiel
     if (!frame_stride_ok(params)) { set_error("nsb_render_forward: frame_stride out of range"); return 1; }
     if (ra->sampler == 0) {
         if (ra->n_per_ray <= 0 || ra->capacity < ra->n_rays * (int64_t)ra->n_per_ray) { set_error("nsb_render_forward: capacity < n_rays * n_per_ray"); return 1; }
-    } else if (ra->sampler == 1 || ra->sampler == 3) {
+    } else if (ra->sampler == 1) {
         if (!ra->near_planes || !ra->far_planes || !ra->binaries || !ra->aabbs) { set_error("nsb_render_forward: occupancy sampler arguments"); return 1; }
-        if (ra->levels < 1 || ra->levels > 8 || (ra->sampler == 3 && ra->levels != 1)) {
-            set_error("nsb_render_forward: levels must be in [1,8] (1 for the single-launch variant)");
-            return 1;
-        }
+        if (ra->levels < 1 || ra->levels > 8) { set_error("nsb_render_forward: levels must be in [1,8]"); return 1; }
     } else { set_error("nsb_render_forward: unknown sampler"); return 1; }
     uint8_t *ws = reinterpret_cast<uint8_t *>(ra->workspace);
     RenderKArgs K;
@@ -1175,11 +1027,10 @@ extern "C" int nsb_render_forward(const nsb_field_params *params, const nsb_fiel
     K.C.workspace = K.hdr->depth_range;
     K.sampler = ra->sampler; K.n_per_ray = ra->n_per_ray; K.near_plane = ra->near_plane; K.capacity = ra->capacity;
     cudaStream_t st = (cudaStream_t)stream;
-    if (ra->sampler == 3) return deform ? launch_render<true, 1>(K, st) : launch_render<false, 1>(K, st);
     if (ra->sampler == 1) {
         // occupancy march as its own small cooperative launch (count | scan | fill, the count stays on the device), then
-        // field + composite in one: with the marcher inside render_kernel_ws ptxas spills 66-82 instructions in the gather
-        // role of the field phase (tools/spill_report.py); sampler == 3 selects that single-launch variant.
+        // field + composite in one: with the marcher inside render_kernel_ws ptxas spilled 66-82 instructions in the
+        // gather role of the field phase (tools/spill_report.py).
         const int rc = launch_march_occ_coop(K.M, K.packed_info, K.hdr, K.partials, K.capacity, ra->march_scratch, st);
         if (rc) return rc;
         return deform ? launch_render<true, 2>(K, st) : launch_render<false, 2>(K, st);

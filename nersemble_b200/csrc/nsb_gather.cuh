@@ -2,16 +2,6 @@
 #pragma once
 #include "nsb_common.cuh"
 
-#ifndef NSB_PREFETCH_QUADS
-// Quad-ahead L2 prefetch (off by default): more requests in flight need not help when the kernel sits at the memory
-// system's REQUEST throughput for this access pattern (tools/randgather.cu measures the random-line rate), and every
-// prefetched line is requested twice.
-#define NSB_PREFETCH_QUADS 0
-#endif
-#ifndef NSB_STREAM_HASHED
-#define NSB_STREAM_HASHED 0   // L1::no_allocate on the hashed levels (off: they DO hit in L1 -- 4 lanes share a sector pair, neighbouring samples share corners)
-#endif
-
 namespace nsb {
 
 // -------------------------------------------------------------------------------------------
@@ -149,98 +139,13 @@ __device__ __forceinline__ void ldg256(const void *p, uint32_t (&r)[8]) {
                  : "l"(p));
 }
 
-// same, streaming: the line is not allocated in L1.  Hashed (fine) levels have no reuse between samples, and keeping
-// them out of L1 leaves it to the dense levels' lines, the code rows and the stack.
-__device__ __forceinline__ void ldg256_stream(const void *p, uint32_t (&r)[8]) {
-    asm volatile("ld.global.nc.L1::no_allocate.v4.b32 {%0,%1,%2,%3}, [%8];\n\t"
-                 "ld.global.nc.L1::no_allocate.v4.b32 {%4,%5,%6,%7}, [%8+16];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                 : "l"(p));
-}
-
-template <int T>
-__device__ __forceinline__ void gather_issue(const nsb_field_params &P, const uint8_t *tab, float x, float y, float z,
-                                             uint32_t dx, uint32_t dy, uint32_t dz, GatherTile &G) {
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-        constexpr int dummy = 0; (void)dummy;
-        const int l = 2 * T + i;
-        const float scale = P.levels.scale[l];
-        const uint32_t res = P.levels.res[l], ent = P.levels.entries[l], off = P.levels.offset[l];
-        const float px = fmaf(scale, x, 0.5f), py = fmaf(scale, y, 0.5f), pz = fmaf(scale, z, 0.5f);
-        const float flx = floorf(px), fly = floorf(py), flz = floorf(pz);
-        const float fx = px - flx, fy = py - fly, fz = pz - flz;
-        const uint32_t cx = (uint32_t)(int)flx + dx, cy = (uint32_t)(int)fly + dy, cz = (uint32_t)(int)flz + dz;
-        G.w[i] = ((dx ? fx : 1.0f - fx) * (dy ? fy : 1.0f - fy)) * (dz ? fz : 1.0f - fz);
-        uint32_t idx;
-        if (P.levels.hashed[l]) {
-            idx = (cx ^ (cy * kPrimeY) ^ (cz * kPrimeZ)) & (ent - 1);   // hashed levels: entries = 2^log2T
-        } else {
-            idx = cx + cy * res + cz * res * res;                         // < 2*entries: `% entries` is one subtract
-            idx = idx >= ent ? idx - ent : idx;
-        }
-        ldg256(tab + (size_t)(off + idx) * 128, G.v[i]);
-    }
-}
-
-// 4 HMMAs + corner-weight scaling + the butterfly stages over lane bits 2 (feat) and 3 (level parity)
-__device__ __forceinline__ float gather_consume(const GatherTile &G, const BlendB &B, int lane) {
-    float c[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-    for (int s = 0; s < 4; ++s) {
-        const uint32_t a[4] = {G.v[0][s], G.v[1][s], G.v[0][4 + s], G.v[1][4 + s]};
-        mma16816(c, a, B.lo[s], B.hi[s]);
-    }
-    const float u0 = butterfly(c[0] * G.w[0], c[1] * G.w[0], 2, lane);
-    const float u1 = butterfly(c[2] * G.w[1], c[3] * G.w[1], 2, lane);
-    return butterfly(u0, u1, 3, lane);
-}
-
-// Software-pipelined gather of one sample: the loads of m-tile t+1 (and, at the end, of the NEXT
-// sample's m-tile 0) are issued before m-tile t is consumed, so every warp always has 4-8 LDG.128
-// in flight.  Ga must already hold this sample's m-tile 0; on return it holds the next sample's
-// m-tile 0 (if has_next).  Returns feature `lane` (= level*2+feat) in every lane.
-__device__ __forceinline__ float gather_sample_pipelined(const nsb_field_params &P, const uint8_t *tab, float x,
-                                                         float y, float z, bool has_next, float nx, float ny, float nz,
-                                                         const BlendB &B, GatherTile &Ga, int lane) {
-    const int g = lane >> 2;
-    const uint32_t dx = g & 1, dy = (g >> 1) & 1, dz = g >> 2;
-    GatherTile Gb;
-    float yv[4];
-    float e, o;
-    gather_issue<1>(P, tab, x, y, z, dx, dy, dz, Gb); e = gather_consume(Ga, B, lane);
-    gather_issue<2>(P, tab, x, y, z, dx, dy, dz, Ga); o = gather_consume(Gb, B, lane); yv[0] = butterfly(e, o, 4, lane);
-    gather_issue<3>(P, tab, x, y, z, dx, dy, dz, Gb); e = gather_consume(Ga, B, lane);
-    gather_issue<4>(P, tab, x, y, z, dx, dy, dz, Ga); o = gather_consume(Gb, B, lane); yv[1] = butterfly(e, o, 4, lane);
-    gather_issue<5>(P, tab, x, y, z, dx, dy, dz, Gb); e = gather_consume(Ga, B, lane);
-    gather_issue<6>(P, tab, x, y, z, dx, dy, dz, Ga); o = gather_consume(Gb, B, lane); yv[2] = butterfly(e, o, 4, lane);
-    gather_issue<7>(P, tab, x, y, z, dx, dy, dz, Gb); e = gather_consume(Ga, B, lane);
-    if (has_next) gather_issue<0>(P, tab, nx, ny, nz, dx, dy, dz, Ga);
-    o = gather_consume(Gb, B, lane); yv[3] = butterfly(e, o, 4, lane);
-    // lanes (g, q==0) hold out[8k+g] in yv[k]; deliver out[lane] to every lane
-    const int src = (lane & 7) * 4;
-    const float s0 = __shfl_sync(0xffffffffu, yv[0], src), s1 = __shfl_sync(0xffffffffu, yv[1], src);
-    const float s2 = __shfl_sync(0xffffffffu, yv[2], src), s3 = __shfl_sync(0xffffffffu, yv[3], src);
-    const int k = lane >> 3;
-    return k == 0 ? s0 : (k == 1 ? s1 : (k == 2 ? s2 : s3));
-}
-
-__device__ __forceinline__ float gather_blend_mma(const nsb_field_params &P, float x, float y, float z,
-                                                  const BlendB &B, int lane) {
-    const int g = lane >> 2, q = lane & 3;
-    const uint8_t *tab = reinterpret_cast<const uint8_t *>(P.tables) + q * 32;
-    GatherTile Ga;
-    gather_issue<0>(P, tab, x, y, z, g & 1, (g >> 1) & 1, g >> 2, Ga);
-    return gather_sample_pipelined(P, tab, x, y, z, false, 0.f, 0.f, 0.f, B, Ga, lane);
-}
-
 // -------------------------------------------------------------------------------------------
 // Quad-cooperative index computation (warp-specialised kernel).
-// In gather_issue every lane of a quad (q = 0..3, the four 32 B pieces of one 128 B line) repeats the same
-// position -> corner -> hash/stride -> trilinear-weight arithmetic for its corner g: 4x redundant, ~80 instructions per
-// level and lane, and the gather warps are issue-limited.  Here the 32 lanes compute 32 DISTINCT (level, corner) pairs -- lane L: level 4U + (L >> 3), corner L & 7 --
-// once per four levels, and each tile's issue fetches the two (entry, weight) pairs it needs with shuffles.
-// Same per-pair arithmetic in the same order as gather_issue: bit-identical results.
+// The four lanes of a quad (q = 0..3, the four 32 B pieces of one 128 B line) need the same position -> corner ->
+// hash/stride -> trilinear-weight arithmetic for their corner g; computed per lane that is 4x redundant, ~80 instructions
+// per level and lane, and the gather warps are issue-limited.  Here the 32 lanes compute 32 DISTINCT (level, corner)
+// pairs -- lane L: level 4U + (L >> 3), corner L & 7 -- once per four levels, and each tile's issue fetches the two
+// (entry, weight) pairs it needs with shuffles.
 // -------------------------------------------------------------------------------------------
 struct QuadIdx {
     uint32_t entry;   // offset[level] + index: absolute table line of (level 4U + (lane >> 3), corner lane & 7)
@@ -272,19 +177,10 @@ __device__ __forceinline__ void gather_issue_q(const nsb_field_params &P, const 
                                                GatherTile &G) {
     const uint32_t e0 = __shfl_sync(0xffffffffu, Q.entry, (2 * J) * 8 + g);
     const uint32_t e1 = __shfl_sync(0xffffffffu, Q.entry, (2 * J + 1) * 8 + g);
-#if !NSB_PREFETCH_QUADS
     G.w[0] = __shfl_sync(0xffffffffu, Q.w, (2 * J) * 8 + g);
     G.w[1] = __shfl_sync(0xffffffffu, Q.w, (2 * J + 1) * 8 + g);
-#endif
-#if NSB_STREAM_HASHED
-    if (P.levels.hashed[4 * U + 2 * J]) ldg256_stream(tab + (size_t)e0 * 128, G.v[0]);   // uniform (constant bank)
-    else ldg256(tab + (size_t)e0 * 128, G.v[0]);
-    if (P.levels.hashed[4 * U + 2 * J + 1]) ldg256_stream(tab + (size_t)e1 * 128, G.v[1]);
-    else ldg256(tab + (size_t)e1 * 128, G.v[1]);
-#else
     ldg256(tab + (size_t)e0 * 128, G.v[0]);
     ldg256(tab + (size_t)e1 * 128, G.v[1]);
-#endif
 }
 
 // Software-pipelined gather of one sample, quad-cooperative.  On entry Ga holds the loads of this sample's tile 0
@@ -325,13 +221,6 @@ __device__ __forceinline__ float gather_consume(const GatherTile &G, const Blend
     return butterfly(u0, u1, 3, lane);
 }
 
-// L2 prefetch of a quad's 32 lines (hashed levels only: the dense levels mostly hit L1/L2 anyway).  Costs no registers
-// beyond the address; issued one quad ahead so that the loads that land in registers find their line in L2.
-__device__ __forceinline__ void quad_prefetch(const nsb_field_params &P, const uint8_t *tab_base, const QuadIdx &Q, int U, int lane) {
-    if (P.levels.hashed[4 * U + (lane >> 3)])
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(tab_base + (size_t)Q.entry * 128));
-}
-
 template <bool CV, class BT>
 __device__ __forceinline__ void gather_sample_quad(const nsb_field_params &P, const uint8_t *tab, float x, float y,
                                                    float z, const float4 *next_xs, float4 &next_out, const BT &B,
@@ -340,45 +229,6 @@ __device__ __forceinline__ void gather_sample_quad(const nsb_field_params &P, co
     const bool owner = (lane & 3) == 0;
     GatherTile Gb;
     float e, o, yv;
-#if NSB_PREFETCH_QUADS
-    // Index computation runs ONE QUAD AHEAD of the loads: quad u+1 is computed (and its lines prefetched into L2) one to
-    // two consume steps before its first load.  Qa / Qb alternate; the tiles do not carry their trilinear weights any
-    // more (the consume step shuffles them out of the quad that produced the tile), so the second QuadIdx is register-neutral.
-    const uint8_t *tb = reinterpret_cast<const uint8_t *>(P.tables);
-    QuadIdx &Qa = Q;
-    QuadIdx Qb;
-#define NSB_W(QQ, J) Ga_w0 = __shfl_sync(0xffffffffu, (QQ).w, (2 * (J)) * 8 + g); Ga_w1 = __shfl_sync(0xffffffffu, (QQ).w, (2 * (J) + 1) * 8 + g)
-    float Ga_w0, Ga_w1;
-    Qb = quad_compute<1>(P, x, y, z, lane); quad_prefetch(P, tb, Qb, 1, lane);
-    gather_issue_q<0, 1>(P, tab, Qa, g, Gb); NSB_W(Qa, 0); Ga.w[0] = Ga_w0; Ga.w[1] = Ga_w1;
-    e = gather_consume(Ga, B, lane, CV ? cv_row + 0 : nullptr);
-    gather_issue_q<1, 0>(P, tab, Qb, g, Ga); NSB_W(Qa, 1); Gb.w[0] = Ga_w0; Gb.w[1] = Ga_w1;
-    o = gather_consume(Gb, B, lane, CV ? cv_row + 16 : nullptr); yv = butterfly(e, o, 4, lane);
-    if (owner) feat_row[g] = __float2half_rn(yv);
-    Qa = quad_compute<2>(P, x, y, z, lane); quad_prefetch(P, tb, Qa, 2, lane);
-    gather_issue_q<1, 1>(P, tab, Qb, g, Gb); NSB_W(Qb, 0); Ga.w[0] = Ga_w0; Ga.w[1] = Ga_w1;
-    e = gather_consume(Ga, B, lane, CV ? cv_row + 32 : nullptr);
-    gather_issue_q<2, 0>(P, tab, Qa, g, Ga); NSB_W(Qb, 1); Gb.w[0] = Ga_w0; Gb.w[1] = Ga_w1;
-    o = gather_consume(Gb, B, lane, CV ? cv_row + 48 : nullptr); yv = butterfly(e, o, 4, lane);
-    if (owner) feat_row[8 + g] = __float2half_rn(yv);
-    Qb = quad_compute<3>(P, x, y, z, lane); quad_prefetch(P, tb, Qb, 3, lane);
-    gather_issue_q<2, 1>(P, tab, Qa, g, Gb); NSB_W(Qa, 0); Ga.w[0] = Ga_w0; Ga.w[1] = Ga_w1;
-    e = gather_consume(Ga, B, lane, CV ? cv_row + 64 : nullptr);
-    gather_issue_q<3, 0>(P, tab, Qb, g, Ga); NSB_W(Qa, 1); Gb.w[0] = Ga_w0; Gb.w[1] = Ga_w1;
-    o = gather_consume(Gb, B, lane, CV ? cv_row + 80 : nullptr); yv = butterfly(e, o, 4, lane);
-    if (owner) feat_row[16 + g] = __float2half_rn(yv);
-    if (next_xs) {
-        next_out = *next_xs;
-        Qa = quad_compute<0>(P, next_out.x, next_out.y, next_out.z, lane); quad_prefetch(P, tb, Qa, 0, lane);
-    }
-    gather_issue_q<3, 1>(P, tab, Qb, g, Gb); NSB_W(Qb, 0); Ga.w[0] = Ga_w0; Ga.w[1] = Ga_w1;
-    e = gather_consume(Ga, B, lane, CV ? cv_row + 96 : nullptr);
-    if (next_xs) gather_issue_q<0, 0>(P, tab, Qa, g, Ga);
-    NSB_W(Qb, 1); Gb.w[0] = Ga_w0; Gb.w[1] = Ga_w1;
-    o = gather_consume(Gb, B, lane, CV ? cv_row + 112 : nullptr); yv = butterfly(e, o, 4, lane);
-    if (owner) feat_row[24 + g] = __float2half_rn(yv);
-#undef NSB_W
-#else
     gather_issue_q<0, 1>(P, tab, Q, g, Gb); e = gather_consume(Ga, B, lane, CV ? cv_row + 0 : nullptr);
     Q = quad_compute<1>(P, x, y, z, lane);
     gather_issue_q<1, 0>(P, tab, Q, g, Ga); o = gather_consume(Gb, B, lane, CV ? cv_row + 16 : nullptr); yv = butterfly(e, o, 4, lane);
@@ -399,7 +249,6 @@ __device__ __forceinline__ void gather_sample_quad(const nsb_field_params &P, co
     }
     o = gather_consume(Gb, B, lane, CV ? cv_row + 112 : nullptr); yv = butterfly(e, o, 4, lane);
     if (owner) feat_row[24 + g] = __float2half_rn(yv);
-#endif
 }
 
 }  // namespace nsb

@@ -393,20 +393,27 @@ __global__ void __launch_bounds__(kCoopThreads) march_occ_coop_kernel(const __gr
     }
 }
 
+// grid of a cooperative launch of Kernel: every CTA resident, at most 4 per SM and at most 1024 (the scan partials)
+template <auto Kernel>
+static int coop_grid() {
+    static int grid = 0;
+    if (grid == 0) {
+        int dev = 0, sms = 0, per_sm = 0;
+        cudaGetDevice(&dev);
+        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, Kernel, kCoopThreads, 0);
+        grid = std::max(1, std::min(sms * std::max(1, std::min(per_sm, 4)), 1024));
+    }
+    return grid;
+}
+
 int launch_march_occ_coop(const nsb_march_args &M, int64_t *packed_info, nsb_render_ws_header *hdr, int64_t *partials,
                           int64_t capacity, float *scratch, cudaStream_t st) {
     MarchCoopArgs K;
     K.M = M; K.packed_info = packed_info; K.hdr = hdr; K.partials = partials; K.capacity = capacity;
     K.slot = capacity / std::max<int64_t>(M.n_rays, 1);
     K.scratch = K.slot >= 1 ? scratch : nullptr;
-    static int grid = 0;
-    if (grid == 0) {
-        int dev = 0, sms = 0, per_sm = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, march_occ_coop_kernel<1>, kCoopThreads, 0);
-        grid = std::max(1, std::min(sms * std::max(1, std::min(per_sm, 4)), 1024));     // <= 1024 scan partials
-    }
+    const int grid = coop_grid<march_occ_coop_kernel<1>>();
     cudaError_t e = cudaMemsetAsync(hdr, 0, sizeof(nsb_render_ws_header), st);      // barrier, status, reserved[0]
     if (e != cudaSuccess) { set_error("march_occ_coop: memset: %s", cudaGetErrorString(e)); return 2; }
     void *kargs[] = {&K};
@@ -637,14 +644,7 @@ extern "C" int nsb_visibility_compact(const nsb_vis_compact_args *args, void *st
     // mask bytes: behind the counts (the workspace of nsb_vis_compact_workspace_bytes)
     K.mask = ws + 64 + 1024 * sizeof(int64_t) + (((size_t)args->n_rays * sizeof(int32_t) + 63) / 64) * 64;
     cudaStream_t st = (cudaStream_t)stream;
-    static int grid = 0;
-    if (grid == 0) {
-        int dev = 0, sms = 0, per_sm = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, vis_compact_coop_kernel, kCoopThreads, 0);
-        grid = std::max(1, std::min(sms * std::max(1, std::min(per_sm, 4)), 1024));
-    }
+    const int grid = coop_grid<vis_compact_coop_kernel>();
     cudaError_t e = cudaMemsetAsync(K.hdr, 0, sizeof(nsb_render_ws_header), st);
     if (e != cudaSuccess) { set_error("nsb_visibility_compact: memset: %s", cudaGetErrorString(e)); return 2; }
     void *kargs[] = {&K};

@@ -936,14 +936,13 @@ def render_rays(P: NativeParams, origins, directions, ray_times, *, window_hash=
                 use_deformation=True, training=False, sampler: str = "occupancy", n_per_ray: int = 0,
                 near_plane: float = 0.0, near_planes=None, far_planes=None, binaries=None, aabbs=None,
                 step: float = 1e-3, cone_angle: float = 0.0, capacity: Optional[int] = None,
-                disable_initial=True, soft_transition=True, single_launch: bool = False,
-                single_traversal: bool = True, uniform_time: Optional[float] = None, line_gather: bool = False,
+                disable_initial=True, soft_transition=True, single_traversal: bool = True,
+                uniform_time: Optional[float] = None, line_gather: bool = False,
                 want_normals: bool = False) -> RenderResult:
     """The fused inference render (nsb_render_forward): sampler -> field -> composite without a host synchronisation.
     sampler 'fixed' (n_per_ray steps from the box entry: ONE launch) or 'occupancy' (nerfacc march of `binaries`
     [levels,res,res,res] within per-ray near_planes / far_planes: the cooperative march launch + one fused launch;
-    single_launch=True marches inside the fused kernel, levels == 1 only; single_traversal=False: count | scan | fill
-    instead of one traversal into per-ray slots + a packing copy).  Returns the per-ray outputs (rgb, accumulation,
+    single_traversal=False: count | scan | fill instead of one traversal into per-ray slots + a packing copy).  Returns the per-ray outputs (rgb, accumulation,
     depth, deformation, num_samples_per_ray, packed_info); `.packed()` gives the per-sample arrays (one sync).
     capacity: per-sample workspace size; default = an upper bound of the march (rays x ceil(largest diagonal / step) + 2).
     The field gathers member-blended tables (frame_table for a uniform_time, timestep_tables otherwise) unless
@@ -970,8 +969,7 @@ def render_rays(P: NativeParams, origins, directions, ray_times, *, window_hash=
         assert b8.shape[1] == b8.shape[2] == b8.shape[3], "cubic grids only"
         ab = aabbs.detach().to(dev, _F32).reshape(levels, 6).contiguous()
         keep += [near_planes, far_planes, b8, ab]
-        a.sampler = 3 if single_launch else 1
-        single_traversal = single_traversal and not single_launch
+        a.sampler = 1
         a.near_planes, a.far_planes, a.binaries, a.aabbs, a.levels, a.res = _ptr(near_planes), _ptr(far_planes), _ptr(b8), _ptr(ab), levels, res
         if capacity is None:
             diag = float((ab[:, 3:] - ab[:, :3]).norm(dim=-1).max())      # host-side: aabbs is a tiny constant buffer
@@ -1011,7 +1009,7 @@ def render_rays(P: NativeParams, origins, directions, ray_times, *, window_hash=
         return out
     opts = make_opts(window_hash, window_deform, use_deformation, True, disable_initial, soft_transition)
     frame = None
-    if use_deformation and not single_launch and not line_gather:
+    if use_deformation and not line_gather:
         if uniform_time is not None:
             # all rays carry this time (one camera frame): the member blend is hoisted into a per-frame table (frame_table)
             frame = P.frame_table(uniform_time, window_hash, disable_initial, soft_transition)

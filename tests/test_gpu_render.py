@@ -21,7 +21,7 @@ def trained():
 @pytest.fixture(scope="module")
 def trained_mma(trained):
     """The same parameters with the deformation MLP of the inference kernels on mma.sync (NSB_TCGEN05=0): what the
-    single-launch occupancy variant (render_kernel_ws<.,1>) and the training kernels run."""
+    training kernels run, and the render kernel render_kernel_ws<true, .>."""
     return trained[0], native_from_oracle(trained[0], DEV, tcgen05=False)
 
 
@@ -56,15 +56,13 @@ def test_fixed_march_one_launch_is_bit_identical_to_the_three_kernel_path(traine
         assert _same(pk["offsets"], want["offsets"])
 
 
-@pytest.mark.parametrize("single_launch", [False, True, "two_pass"])
+@pytest.mark.parametrize("mode", ["one_traversal", "one_traversal_mma", "count_scan_fill"])
 @pytest.mark.parametrize("levels", [1, 2])
-def test_occupancy_march_fused_is_bit_identical(trained, trained_mma, levels, single_launch):
+def test_occupancy_march_fused_is_bit_identical(trained, trained_mma, levels, mode):
     from nersemble_b200 import ops
     from oracle.gen_golden import blob_grid
     from oracle.tp import nerfacc_cpu
-    if single_launch is True and levels != 1:
-        pytest.skip("the single-launch variant marches single-level grids")
-    P, NP = trained_mma if single_launch is True else trained       # bit-identity holds within one tensor role
+    P, NP = trained_mma if mode == "one_traversal_mma" else trained       # bit-identity holds within one tensor role
     R = 700                                            # > 256 * ... several scan slabs per CTA chunk is covered by R = 40 000 below
     o, d, t = _rays(R, 11)
     d[5] = torch.tensor([0.0, 0.0, -1.0]); o[5] = torch.tensor([0.1, 0.2, 9.0])
@@ -76,11 +74,11 @@ def test_occupancy_march_fused_is_bit_identical(trained, trained_mma, levels, si
     far = torch.full((R,), 1e3, device=DEV)
     ts, te, ri, info = ops.march_occupancy(o, d, near, far, occ, aabbs, 0.011, 0.0)
     want = ops.render_packed(NP, o, d, t, ts, te, ri, info, window_hash=32.0, window_deform=7.0, training=False)
-    # False: cooperative march, ONE traversal into per-ray slots + packing copy (default); "two_pass": count | scan | fill;
-    # True: the march inside the fused kernel
-    kw = dict(single_launch=single_launch is True)
+    # cooperative march launch, then the fused field + composite launch.  "one_traversal": ONE traversal into per-ray
+    # slots + packing copy (the default), wgmma deformation role; "one_traversal_mma": the same on the mma.sync role
+    # (render_kernel_ws<true, 2>); "count_scan_fill": the march traverses the grid twice (count | scan | fill)
     got = ops.render_rays(NP, o, d, t, window_hash=32.0, window_deform=7.0, sampler="occupancy", near_planes=near,
-                          far_planes=far, binaries=occ, aabbs=aabbs, step=0.011, single_traversal=single_launch is False, **kw)
+                          far_planes=far, binaries=occ, aabbs=aabbs, step=0.011, single_traversal=mode != "count_scan_fill")
     assert _same(got["packed_info"], info)
     for k in ("rgb", "accumulation", "depth", "deformation"):
         assert _same(got[k], want[k]), k

@@ -2,8 +2,7 @@
   3-kernel op path (march_fixed -> field_forward -> composite)      [5 launches]
   ops.render_rays fixed        (ONE launch)
   ops.render_rays occupancy    (cooperative march launch + one fused launch; all-ones grid, fars = 256 steps)
-  ops.render_rays occupancy single_launch=True
-and checks that all four produce the same RGB."""
+and checks that all three produce the same RGB."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch, bench
@@ -30,10 +29,10 @@ near = ops.march_fixed(o, d, P.aabb, 1, bench.STEP, bench.NEAR)[0]
 far = near + bench.SAMPLES_PER_RAY * bench.STEP
 occ = torch.ones((1, 128, 128, 128), dtype=torch.bool, device=dev)
 aabbs = P.aabb.reshape(1, 6).to(dev)
-def occupancy(single=False):
-    return ops.render_rays(P, o, d, t, window_hash=32.0, window_deform=7.0, sampler="occupancy", near_planes=near, far_planes=far, binaries=occ, aabbs=aabbs, step=bench.STEP, single_launch=single, capacity=R * (bench.SAMPLES_PER_RAY + 2))
+def occupancy():
+    return ops.render_rays(P, o, d, t, window_hash=32.0, window_deform=7.0, sampler="occupancy", near_planes=near, far_planes=far, binaries=occ, aabbs=aabbs, step=bench.STEP, capacity=R * (bench.SAMPLES_PER_RAY + 2))
 ref = three()["rgb"]
-for name, fn in (("fixed", fixed), ("occupancy", occupancy), ("occupancy_single", lambda: occupancy(True))):
+for name, fn in (("fixed", fixed), ("occupancy", occupancy)):
     out = fn(); torch.cuda.synchronize()
     print(name, "max |rgb - 3kernel|", float((out["rgb"] - ref).abs().max()), "n_total", int(out["_buffers"]["header"][2]))
-print(f"ms: three_kernel {timeit(three):.3f}  fixed_1launch {timeit(fixed):.3f}  occupancy_2launch {timeit(occupancy):.3f}  occupancy_1launch {timeit(lambda: occupancy(True)):.3f}")
+print(f"ms: three_kernel {timeit(three):.3f}  fixed_1launch {timeit(fixed):.3f}  occupancy_2launch {timeit(occupancy):.3f}")
