@@ -27,6 +27,8 @@
  *   nsb_composite_backward / nsb_field_backward / nsb_deform_backward
  *                          torch autograd through all of the above (training; with per-sample conditioning codes also
  *                          for the stand-alone field and deformation modules of the component API)
+ *   nsb_deform_input_grad  torch.autograd.grad of SE3DeformationField.compute_offsets with respect to its input
+ *                          positions (an extension: the reference never differentiates the warp by position)
  *   nsb_table_adam_step    torch.optim.Adam on the 8 tcnn grid tensors (scripts/train/train_nersemble.py:243-247) and
  *                          tcnn's per-call fp32 -> fp16 cast of the table parameters
  */
@@ -273,6 +275,25 @@ size_t nsb_deform_bwd_workspace_bytes(void);
 int nsb_deform_backward(const nsb_field_params *params, const nsb_field_opts *opts, const nsb_samples *samples,
                         const nsb_deform_bwd_args *args, void *stream);
 
+/* Vector-Jacobian product of the deformation with respect to its INPUT position: d_pn = J^T u per sample, with
+ * offset(p_n) = R(p_n) p_n + V v - p_n the normalised offsets nsb_field_forward writes, p_n the normalised sample position
+ * and J = d offset / d p_n through the windowed positional encoding (opts->pe_window), the six stem layers, both heads,
+ * the SE(3) exponential map and the direct dependence (R - I) p_n.  The stem forward is recomputed per tile with the
+ * field kernels' operand rounding (nothing saved by a forward is needed); warp codes enter as params->deform_code_bias
+ * or samples->sample_code_bias.  A row whose warp is NaN (replaced by the identity in the forward) gets 0.  The deltas
+ * are fp16 MMA operands: u is multiplied by loss_scale and the result divided by it.  No atomics: bit-identical from run
+ * to run.  Samples beyond *n_samples_dev (when given) are not touched.  Not differentiable. */
+typedef struct {
+    const void *deform_packed_t;     /* fp16 TRANSPOSED stem/head weights (python: pack_deform_bwd) */
+    const void *deform_packed_pe_t;  /* fp16 TRANSPOSED posenc columns of layers 0 and 4, two [128 -> 48] blocks in MMA-B
+                                        fragment order (python: pack_deform_pe_t; 24576 bytes) */
+    const float *u;                  /* [n][3] cotangent of the normalised offsets */
+    float loss_scale;
+    float *d_pn;                     /* [n][3] out: J^T u, with respect to the NORMALISED input position */
+} nsb_deform_vjp_args;
+int nsb_deform_input_grad(const nsb_field_params *params, const nsb_field_opts *opts, const nsb_samples *samples,
+                          const nsb_deform_vjp_args *args, void *stream);
+
 /* Fused hash-table optimiser step.  Replaces, for the table parameter only, what the reference's training loop does
  * with torch: materialise the dense fp32 gradient of the 8 tcnn grids, run torch.optim.Adam over it (nerfstudio
  * AdamOptimizerConfig, eps 1e-15: train_nersemble.py optimizers["fields"]) and let tcnn re-read the parameters.  One
@@ -424,11 +445,20 @@ int nsb_render_forward(const nsb_field_params *params, const nsb_field_opts *opt
  *   n = -normalize(grad_scale * d h0 / d x),  normalize(v) = v / max(|v|, 1e-12)
  * h0 = mlp_base output 0 before trunc_exp; x = the normalised hash-input position after the in-box selector (0 outside
  * the box: such a sample gets the gradient at the box origin), formed exactly as the field kernels form it (with offsets,
- * the normalised offsets added to the world position).  With deformation these are canonical-space normals.  The gather
+ * the normalised offsets added to the world position).  With deformation these are canonical-space normals unless
+ * observation_space is set (below).  The gather
  * reads the tables the field kernels read for the same params / samples: frame_table (one frame or a timestep stack),
  * else the 128 B lines with sample_blend_codes or the timestep's blend codes.  Not differentiable.
  *   out_normals[r] = v / (|v| + 1e-10), v = sum over the ray's packed_info segment of weights[i] * normals[i], summed
- * in a fixed order (bit-identical from run to run).  Samples beyond *n_samples_dev (when given) are not touched. */
+ * in a fixed order (bit-identical from run to run).  Samples beyond *n_samples_dev (when given) are not touched.
+ *
+ * observation_space != 0 (an extension; needs opts->use_deformation, offsets and the deformation weights in params):
+ * the gradient with respect to the OBSERVED position p instead of the warped one.  With p_n the normalised observed
+ * position, D = diag(aabb extent), J as in nsb_deform_input_grad, g = d h0 / d x and s the in-box selector of the warped
+ * position, the hash input is x = s (p_n + D^-1 offset(p_n)), so
+ *   n = -normalize(grad_scale * s * (g + J^T D^-1 g))
+ * A sample whose warped position is outside the box gets the zero vector (s = 0).  Runs the canonical pass with
+ * grad_scale 1, the deformation input gradient of u = D^-1 n into vjp_scratch, and a combine pass over `normals`. */
 typedef struct {
     const float *offsets;        /* [n][3] or NULL (no deformation): the offsets the field / render kernels wrote */
     float grad_scale[3];          /* per-axis factor on d h0 / d x before normalising: 1 (normalised space, the field API)
@@ -438,6 +468,11 @@ typedef struct {
     const float *weights;         /* [n] render weights, needed for out_normals */
     float *normals;               /* [n][3] out; NULL: nothing is computed (required for out_normals) */
     float *out_normals;           /* [n_rays][3] out or NULL */
+    int32_t observation_space;    /* 0: canonical-space normals */
+    float loss_scale;             /* observation space: nsb_deform_vjp_args.loss_scale */
+    const void *deform_packed_t;  /* observation space: nsb_deform_vjp_args.deform_packed_t */
+    const void *deform_packed_pe_t; /* observation space: nsb_deform_vjp_args.deform_packed_pe_t */
+    float *vjp_scratch;           /* observation space: [n][3] scratch */
 } nsb_normals_args;
 int nsb_normals_forward(const nsb_field_params *params, const nsb_field_opts *opts, const nsb_samples *samples,
                         const nsb_normals_args *args, void *stream);

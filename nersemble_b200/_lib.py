@@ -143,7 +143,14 @@ class RayBatchArgs(C.Structure):
 
 class NormalsArgs(C.Structure):     # nsb_normals_args
     _fields_ = [("offsets", C.c_void_p), ("grad_scale", C.c_float * 3), ("packed_info", C.c_void_p), ("n_rays", C.c_int64),
-                ("weights", C.c_void_p), ("normals", C.c_void_p), ("out_normals", C.c_void_p)]
+                ("weights", C.c_void_p), ("normals", C.c_void_p), ("out_normals", C.c_void_p),
+                ("observation_space", C.c_int32), ("loss_scale", C.c_float), ("deform_packed_t", C.c_void_p),
+                ("deform_packed_pe_t", C.c_void_p), ("vjp_scratch", C.c_void_p)]
+
+
+class DeformVjpArgs(C.Structure):   # nsb_deform_vjp_args
+    _fields_ = [("deform_packed_t", C.c_void_p), ("deform_packed_pe_t", C.c_void_p), ("u", C.c_void_p),
+                ("loss_scale", C.c_float), ("d_pn", C.c_void_p)]
 
 
 class RenderWsHeader(C.Structure):
@@ -167,6 +174,8 @@ SYMBOLS = {
     "nsb_deform_bwd_workspace_bytes": (C.c_size_t, []),
     "nsb_deform_backward": (C.c_int, [C.POINTER(FieldParams), C.POINTER(FieldOpts), C.POINTER(Samples),
                                       C.POINTER(DeformBwdArgs), C.c_void_p]),
+    "nsb_deform_input_grad": (C.c_int, [C.POINTER(FieldParams), C.POINTER(FieldOpts), C.POINTER(Samples),
+                                        C.POINTER(DeformVjpArgs), C.c_void_p]),
     "nsb_losses_forward": (C.c_int, [C.POINTER(LossArgs), C.c_void_p]),
     "nsb_losses_backward": (C.c_int, [C.POINTER(LossArgs), C.c_void_p]),
     "nsb_table_adam_step": (C.c_int, [C.POINTER(TableAdamArgs), C.c_void_p]),

@@ -18,6 +18,11 @@ int num_sms();
 // check_samples: a sample source, and ray-based samples with all of directions, t_starts, t_ends, ray_indices.
 int check_field_params(const char *who, const nsb_field_params *p);
 int check_samples(const char *who, const nsb_samples *s);
+// nsb_deform_vjp.cu: d_pn = J^T (u_scale * u) of the deformation (nsb_deform_input_grad) after the entry point's own
+// checks; errors are prefixed by `who`.
+int launch_deform_input_grad(const char *who, const nsb_field_params *params, const nsb_field_opts *opts,
+                             const nsb_samples *samples, const nsb_deform_vjp_args *args, const float u_scale[3],
+                             cudaStream_t st);
 // nsb_render.cu: the occupancy march as ONE cooperative launch (count | scan | fill); leaves packed_info, the packed
 // samples (below `capacity`) and, in the workspace header, n_total / status.  Zeroes and uses hdr->barrier.
 int launch_march_occ_coop(const nsb_march_args &M, int64_t *packed_info, nsb_render_ws_header *hdr, int64_t *partials,

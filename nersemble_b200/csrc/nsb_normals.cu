@@ -9,6 +9,8 @@
 // the level scale, the math of the position gradient in nsb_backward.cu); the two z halves meet in one shuffle, after
 // which lane j holds feature j and d feat_j / d x.  mlp_base layer 0 runs in fp32 FMAs from shared memory for the ReLU
 // mask, d h0 / d feat = W0^T (W1[0] . mask), and a warp sum contracts it with d feat / d x.
+// normals_observation_kernel (observation_space): one thread per sample turns the unit canonical normal n and
+// d = J^T D^-1 n (nsb_deform_vjp.cu) into n_obs = normalize(grad_scale * s * (n + d)); n already carries the minus sign.
 // normals_composite_kernel: one warp per ray sums w_i * n_i over its packed segment in a fixed order (no atomics).
 #include <algorithm>
 
@@ -183,6 +185,38 @@ __global__ void __launch_bounds__(kNrmWarps * 32) normals_kernel(const __grid_co
     }
 }
 
+// Observation-space normals from the canonical ones: the chain rule through x = s * (p_n + D^-1 offset(p_n)).  The warped
+// position and its in-box selector s are formed as normals_kernel forms them.
+__global__ void __launch_bounds__(256) normals_observation_kernel(const __grid_constant__ NormalsKArgs K) {
+    const int64_t n = K.S.n_samples_dev ? min(*K.S.n_samples_dev, K.S.n_samples) : K.S.n_samples;
+    for (int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; s < n; s += (int64_t)gridDim.x * blockDim.x) {
+        float px, py, pz;
+        if (K.S.origins) {
+            const int64_t ri = K.S.ray_indices[s];
+            const float mid = __fadd_rn(K.S.t_starts[s], K.S.t_ends[s]);
+            px = ray_midpoint(K.S.origins[3 * ri + 0], K.S.directions[3 * ri + 0], mid);
+            py = ray_midpoint(K.S.origins[3 * ri + 1], K.S.directions[3 * ri + 1], mid);
+            pz = ray_midpoint(K.S.origins[3 * ri + 2], K.S.directions[3 * ri + 2], mid);
+        } else {
+            px = K.S.positions[3 * s + 0]; py = K.S.positions[3 * s + 1]; pz = K.S.positions[3 * s + 2];
+        }
+        px = __fadd_rn(px, K.N.offsets[3 * s + 0]);
+        py = __fadd_rn(py, K.N.offsets[3 * s + 1]);
+        pz = __fadd_rn(pz, K.N.offsets[3 * s + 2]);
+        const float x = box_coord(px, K.P.aabb[0], K.aabb_size[0]);
+        const float y = box_coord(py, K.P.aabb[1], K.aabb_size[1]);
+        const float z = box_coord(pz, K.P.aabb[2], K.aabb_size[2]);
+        const bool sel = (x > 0.f) && (x < 1.f) && (y > 0.f) && (y < 1.f) && (z > 0.f) && (z < 1.f);
+        float v[3];
+#pragma unroll
+        for (int k = 0; k < 3; ++k)
+            v[k] = sel ? K.N.grad_scale[k] * (K.N.normals[3 * s + k] + K.N.vjp_scratch[3 * s + k]) : 0.f;
+        const float den = fmaxf(sqrtf(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]), 1e-12f);
+#pragma unroll
+        for (int k = 0; k < 3; ++k) K.N.normals[3 * s + k] = v[k] / den;
+    }
+}
+
 // NormalsRenderer(normalize=True): N = v / (|v| + 1e-10), v = sum_i w_i n_i over the ray's samples.  Each lane sums a fixed
 // stride of the segment, then a fixed butterfly: the result is the same bits on every run.
 __global__ void __launch_bounds__(256) normals_composite_kernel(const __grid_constant__ NormalsKArgs K) {
@@ -227,15 +261,34 @@ extern "C" int nsb_normals_forward(const nsb_field_params *params, const nsb_fie
         set_error("nsb_normals_forward: tables / blend codes missing");
         return 1;
     }
+    const bool observation = args->observation_space != 0;
+    if (observation && (!opts->use_deformation || !args->offsets || !args->vjp_scratch)) {
+        set_error("nsb_normals_forward: observation_space needs use_deformation, offsets and vjp_scratch");
+        return 1;
+    }
     if (samples->n_samples <= 0) return 0;
     NormalsKArgs K;
     K.P = *params; K.O = *opts; K.S = *samples; K.N = *args;
     for (int k = 0; k < 3; ++k) K.aabb_size[k] = params->aabb[3 + k] - params->aabb[k];
     cudaStream_t st = (cudaStream_t)stream;
     const int grid = (int)std::min<int64_t>((samples->n_samples + kNrmWarps - 1) / kNrmWarps, (int64_t)num_sms() * 8);
+    if (observation)        // the canonical pass leaves -g / |g| of the normalised hash input; grad_scale applies at the end
+        for (int k = 0; k < 3; ++k) K.N.grad_scale[k] = 1.0f;
     if (frame) normals_kernel<true><<<grid, kNrmWarps * 32, 0, st>>>(K);
     else normals_kernel<false><<<grid, kNrmWarps * 32, 0, st>>>(K);
     int rc = check_launch("normals_kernel");
+    if (!rc && observation) {
+        nsb_deform_vjp_args V;
+        V.deform_packed_t = args->deform_packed_t; V.deform_packed_pe_t = args->deform_packed_pe_t;
+        V.u = args->normals; V.loss_scale = args->loss_scale; V.d_pn = args->vjp_scratch;
+        const float inv_extent[3] = {1.0f / K.aabb_size[0], 1.0f / K.aabb_size[1], 1.0f / K.aabb_size[2]};
+        rc = launch_deform_input_grad("nsb_normals_forward", params, opts, samples, &V, inv_extent, st);
+        if (rc) return rc;
+        for (int k = 0; k < 3; ++k) K.N.grad_scale[k] = args->grad_scale[k];
+        const int ogrid = (int)std::min<int64_t>((samples->n_samples + 255) / 256, (int64_t)num_sms() * 8);
+        normals_observation_kernel<<<ogrid, 256, 0, st>>>(K);
+        rc = check_launch("normals_observation_kernel");
+    }
     if (rc || !args->out_normals || args->n_rays == 0) return rc;
     const int rgrid = (int)std::min<int64_t>((args->n_rays + 7) / 8, (int64_t)num_sms() * 8);
     normals_composite_kernel<<<rgrid, 256, 0, st>>>(K);

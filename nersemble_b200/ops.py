@@ -87,6 +87,7 @@ class NativeParams:
     deform_code_w: Optional[list] = None              # (stem_w[0], stem_w[4], stem_b[0], stem_b[4]): per-sample code bias
     deform_code_bias: Optional[torch.Tensor] = None   # float [T, 2, 128]
     deform_packed_umma: Optional[torch.Tensor] = None # half, wgmma core-matrix order (inference kernels; opt-in)
+    deform_packed_pe_t: Optional[torch.Tensor] = None # half, transposed posenc columns of layers 0 / 4 (deform_input_grad)
 
     def __post_init__(self):
         self.aabb_list = [float(v) for v in self.aabb.detach().cpu().reshape(-1)]
@@ -178,6 +179,14 @@ class NativeParams:
             self._stack = cached = (key, out)
         return cached[1]
 
+    def pe_t(self) -> torch.Tensor:
+        """packing.pack_deform_pe_t of the stem weights, packed on first use (only the deformation input gradient reads it)."""
+        if self.deform_packed_pe_t is None:
+            if self.deform_code_w is None:
+                raise RuntimeError("the deformation input gradient needs deformation weights (NativeParams.build(deform=...))")
+            self.deform_packed_pe_t = packing.pack_deform_pe_t(self.deform_code_w[0], self.deform_code_w[1])
+        return self.deform_packed_pe_t
+
     def c_params(self, inference: bool = False, frame: Optional[torch.Tensor] = None) -> _lib.FieldParams:
         """inference: the call saves nothing for a backward pass -- the kernels may then run the deformation MLP on
         wgmma, which takes its weights in another order (packed here on first use: a training step never pays).
@@ -255,14 +264,7 @@ def field_forward(P: NativeParams, *, window_hash=None, window_deform=None, use_
     if sample_blend_codes is not None:
         assert tuple(sample_blend_codes.shape) == (n, 32)
     if sample_warp_codes is not None:
-        # component API (SE3DeformationField.compute_offsets with explicit codes): the kernel takes the code columns of
-        # layers 0 / 4 as a per-sample bias, W_code . code + b (fp16-rounded operands, fp32 accumulate)
-        assert sample_warp_codes.shape == (n, 128) and P.deform_code_w is not None
-        if n > (1 << 24):
-            raise RuntimeError("per-sample warp codes: at most 2^24 samples per call")
-        w0, w4, b0, b4 = P.deform_code_w
-        scb = packing.deform_code_bias({0: w0, 4: w4}, {0: b0, 4: b4}, sample_warp_codes.to(dev))
-        s.sample_code_bias = _ptr(scb); keep.append(scb)
+        _fill_sample_code_bias(P, s, keep, sample_warp_codes, n, dev)
     if n_samples_dev is not None:      # the arrays hold `n` slots, the device scalar says how many are samples (no host sync)
         assert n_samples_dev.dtype == torch.int64 and n_samples_dev.is_cuda and n_samples_dev.numel() == 1
         s.n_samples_dev = _ptr(n_samples_dev); keep.append(n_samples_dev)
@@ -308,6 +310,61 @@ def field_forward(P: NativeParams, *, window_hash=None, window_deform=None, use_
     return out
 
 
+def _fill_sample_code_bias(P: NativeParams, s, keep, sample_warp_codes, n: int, dev) -> None:
+    """Component API (explicit per-sample warp codes): the kernels take the code columns of layers 0 / 4 as a per-sample
+    bias, W_code . code + b (fp16-rounded operands, fp32 accumulate)."""
+    assert sample_warp_codes.shape == (n, 128) and P.deform_code_w is not None
+    if n > (1 << 24):
+        raise RuntimeError("per-sample warp codes: at most 2^24 samples per call")
+    w0, w4, b0, b4 = P.deform_code_w
+    scb = packing.deform_code_bias({0: w0, 4: w4}, {0: b0, 4: b4}, sample_warp_codes.to(dev))
+    s.sample_code_bias = _ptr(scb); keep.append(scb)
+
+
+# Scale of the fp16 deltas of the deformation input gradient.  Its cotangents are unit normals over the box extent or
+# caller vectors of similar size, and the chain only shrinks them (head weights << 1): 1024 keeps the deltas in fp16's
+# normal range without coming near its maximum.
+VJP_LOSS_SCALE = 1024.0
+NORMAL_SPACES = ("canonical", "observation")
+
+
+def deform_input_grad(P: NativeParams, u: torch.Tensor, *, window_deform=None, loss_scale: float = VJP_LOSS_SCALE,
+                      sample_warp_codes: Optional[torch.Tensor] = None, n_samples_dev: Optional[torch.Tensor] = None,
+                      out: Optional[torch.Tensor] = None, **sample_kw) -> torch.Tensor:
+    """J^T u [n,3] of the SE(3) deformation with respect to its NORMALISED input position (nsb_deform_input_grad):
+    offset(p_n) = field_forward(...)["offsets"], J = d offset / d p_n through the windowed positional encoding, the stem,
+    both heads, the exponential map and the direct term (R - I) p_n.  u [n,3]: cotangent of the normalised offsets.
+    Samples as in field_forward (positions / sample_times, or origins / directions / t_starts / t_ends / ray_indices /
+    ray_times), with table warp codes or sample_warp_codes [n,128].  Written into `out` (float32 [n,3], contiguous) when
+    given; rows beyond *n_samples_dev are not touched.
+    Nothing a forward saved is needed; not differentiable."""
+    keep: list = []
+    s = _lib.Samples()
+    n = _fill_samples(s, keep, **sample_kw)
+    u = _f32c(u).reshape(-1, 3)
+    _need_cuda(u)
+    assert u.shape[0] == n, (u.shape, n)
+    dev = u.device
+    if sample_warp_codes is not None:
+        _fill_sample_code_bias(P, s, keep, sample_warp_codes, n, dev)
+    if n_samples_dev is not None:
+        assert n_samples_dev.dtype == torch.int64 and n_samples_dev.is_cuda and n_samples_dev.numel() == 1
+        s.n_samples_dev = _ptr(n_samples_dev); keep.append(n_samples_dev)
+    if out is None:
+        out = _rows(n, (3,), _F32, dev)
+    assert out.dtype == _F32 and out.is_cuda and out.is_contiguous() and tuple(out.shape) == (n, 3)
+    if n == 0:
+        return out
+    a = _lib.DeformVjpArgs()
+    a.deform_packed_t, a.deform_packed_pe_t = _ptr(P.deform_packed_t), _ptr(P.pe_t())
+    a.u, a.loss_scale, a.d_pn = _ptr(u), float(loss_scale), _ptr(out)
+    opts = make_opts(None, window_deform, True, False)
+    cp = P.c_params()
+    _lib.check(_lib.load().nsb_deform_input_grad(C.byref(cp), C.byref(opts), C.byref(s), C.byref(a), _stream()),
+               "nsb_deform_input_grad")
+    return out
+
+
 def _world_grad_scale(P: NativeParams):
     """Per-axis factor that turns d h0 / d(normalised position) into d h0 / d(world position): 1 / aabb extent."""
     a = P.aabb_list
@@ -315,11 +372,16 @@ def _world_grad_scale(P: NativeParams):
 
 
 def _normals_launch(P: NativeParams, cp, opts, s, n_samples: int, dev, *, offsets=None, grad_scale=(1.0, 1.0, 1.0),
-                    packed_info=None, weights=None, keep=None) -> Dict[str, torch.Tensor]:
+                    packed_info=None, weights=None, keep=None, observation: bool = False) -> Dict[str, torch.Tensor]:
     """nsb_normals_forward on filled nsb_samples: per-sample normals [n, 3], and with packed_info / weights the per-ray
-    composite `ray_normals` [R, 3]."""
+    composite `ray_normals` [R, 3].  observation: apply the deformation Jacobian (needs offsets and, in opts, the
+    deformation window)."""
     a = _lib.NormalsArgs()
     keep = list(keep or [])
+    if observation:
+        a.observation_space, a.loss_scale = 1, VJP_LOSS_SCALE
+        a.deform_packed_t, a.deform_packed_pe_t = _ptr(P.deform_packed_t), _ptr(P.pe_t())
+        a.vjp_scratch = _ptr(_workspace("normals_vjp", max(n_samples, 1) * 12, dev))
     if offsets is not None:
         offsets = _f32c(offsets).reshape(-1, 3)
         _need_cuda(offsets)
@@ -347,7 +409,8 @@ def field_normals(P: NativeParams, *, window_hash=None, offsets: Optional[torch.
                   positions=None, sample_times=None, sample_blend_codes=None, n_samples_dev: Optional[torch.Tensor] = None,
                   uniform_time: Optional[float] = None, line_gather: bool = False, world_space: bool = False,
                   packed_info: Optional[torch.Tensor] = None, weights: Optional[torch.Tensor] = None,
-                  disable_initial: bool = True, soft_transition: bool = True) -> Dict[str, torch.Tensor]:
+                  disable_initial: bool = True, soft_transition: bool = True, space: str = "canonical",
+                  window_deform=None, sample_warp_codes: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
     """Surface normals of the density field (nsb_normals_forward), nerfstudio's Field.get_normals:
     n = -normalize(d h0 / d x), h0 = mlp_base output 0 before trunc_exp, x = the normalised hash-input position after the
     in-box selector (outside the box x = 0, and the normal is the gradient at the box origin).  Takes the sample keywords
@@ -355,7 +418,13 @@ def field_normals(P: NativeParams, *, window_hash=None, offsets: Optional[torch.
     Jacobian is not applied).  world_space=True divides the gradient by the box extent per axis before normalising.
     With offsets, the tables are gathered as field_forward gathers them for the same call (blended frame table / timestep
     stack unless line_gather or per-sample blend codes).  With packed_info [R,2] and weights [n] also `ray_normals`
-    [R,3] = sum_i w_i n_i / (|sum_i w_i n_i| + 1e-10).  Not differentiable.  Returns {"normals": [n,3], ...}."""
+    [R,3] = sum_i w_i n_i / (|sum_i w_i n_i| + 1e-10).  Not differentiable.  Returns {"normals": [n,3], ...}.
+    space="observation" (with offsets) applies the deformation Jacobian: the gradient with respect to the OBSERVED
+    position, -normalize(s (g + J^T D^-1 g)), zero where the warped position leaves the box (s = 0).  It needs the
+    `window_deform` of the evaluation that produced the offsets, and `sample_warp_codes` if that evaluation took them.
+    Without offsets there is no deformation and both spaces are the same."""
+    if space not in NORMAL_SPACES:
+        raise ValueError(f"space must be one of {NORMAL_SPACES}, got {space!r}")
     keep: list = []
     s = _lib.Samples()
     n = _fill_samples(s, keep, origins=origins, directions=directions, ray_times=ray_times, t_starts=t_starts, t_ends=t_ends,
@@ -370,11 +439,15 @@ def field_normals(P: NativeParams, *, window_hash=None, offsets: Optional[torch.
     frame = None
     if offsets is not None:
         frame = _blended_tables(P, uniform_time, window_hash, disable_initial, soft_transition, line_gather, sample_blend_codes)
-    opts = make_opts(window_hash, None, offsets is not None, False, disable_initial, soft_transition)
+    observation = space == "observation" and offsets is not None
+    if observation and sample_warp_codes is not None:
+        _fill_sample_code_bias(P, s, keep, sample_warp_codes, n, dev)
+    opts = make_opts(window_hash, window_deform if observation else None, offsets is not None, False, disable_initial,
+                     soft_transition)
     cp = P.c_params(inference=frame is not None, frame=frame)
     return _normals_launch(P, cp, opts, s, n, dev, offsets=offsets,
                            grad_scale=_world_grad_scale(P) if world_space else (1.0, 1.0, 1.0),
-                           packed_info=packed_info, weights=weights, keep=keep)
+                           packed_info=packed_info, weights=weights, keep=keep, observation=observation)
 
 
 def _blended_tables(P: NativeParams, uniform_time, window_hash, disable_initial, soft_transition, line_gather=False,
@@ -925,7 +998,7 @@ def render_rays(P: NativeParams, origins, directions, ray_times, *, window_hash=
                 step: float = 1e-3, cone_angle: float = 0.0, capacity: Optional[int] = None,
                 disable_initial=True, soft_transition=True, single_traversal: bool = True,
                 uniform_time: Optional[float] = None, line_gather: bool = False,
-                want_normals: bool = False) -> RenderResult:
+                want_normals: bool = False, normals_space: str = "canonical") -> RenderResult:
     """The fused inference render (nsb_render_forward): sampler -> field -> composite without a host synchronisation.
     sampler 'fixed' (n_per_ray steps from the box entry: ONE launch) or 'occupancy' (nerfacc march of `binaries`
     [levels,res,res,res] within per-ray near_planes / far_planes: the cooperative march launch + one fused launch;
@@ -935,7 +1008,11 @@ def render_rays(P: NativeParams, origins, directions, ray_times, *, window_hash=
     The field gathers member-blended tables (frame_table for a uniform_time, timestep_tables otherwise) unless
     line_gather=True forces the per-sample blend of the 128 B table lines.
     want_normals=True adds `normals` [R,3]: the world-space surface normals of the call's own packed samples (field_normals
-    on the same tables), composited with the render weights and normalised; still without a host synchronisation."""
+    on the same tables), composited with the render weights and normalised; still without a host synchronisation.
+    normals_space="observation" applies the deformation Jacobian to them (field_normals(space=...)); without
+    use_deformation both spaces are the same."""
+    if normals_space not in NORMAL_SPACES:
+        raise ValueError(f"normals_space must be one of {NORMAL_SPACES}, got {normals_space!r}")
     lib = _lib.load()
     origins, directions = _f32c(origins).reshape(-1, 3), _f32c(directions).reshape(-1, 3)
     ray_times = None if ray_times is None else _f32c(ray_times).reshape(-1)
@@ -1007,7 +1084,8 @@ def render_rays(P: NativeParams, origins, directions, ray_times, *, window_hash=
         s.origins, s.directions, s.ray_times = _ptr(origins), _ptr(directions), _ptr(ray_times)
         s.t_starts, s.t_ends, s.ray_indices = _ptr(buf["t_starts"]), _ptr(buf["t_ends"]), _ptr(buf["ray_indices"])
         nrm = _normals_launch(P, cp, opts, s, cap, dev, offsets=buf["offsets"], grad_scale=_world_grad_scale(P),
-                              packed_info=info, weights=buf["weights"])
+                              packed_info=info, weights=buf["weights"],
+                              observation=use_deformation and normals_space == "observation")
         buf["normals"] = nrm["normals"]
         out["normals"] = nrm["ray_normals"]
     return out

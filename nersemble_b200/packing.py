@@ -144,6 +144,22 @@ def pack_deform_bwd(stem_w, r_w, v_w) -> torch.Tensor:
     return packed.contiguous()
 
 
+def pack_deform_pe_t(w0: torch.Tensor, w4: torch.Tensor) -> torch.Tensor:
+    """Transposed posenc columns of stem layers 0 and 4 for nsb_deform_input_grad: two [K = 128 outputs -> N = 48] blocks
+    (N in the kernel's posenc order, deform_input_colmap()[:48]; padding columns are zero), each in MMA-B fragment order
+    with 3 n-tile pairs per k-tile.  pack_deform_bwd only carries the hidden and code columns."""
+    cm = torch.as_tensor(deform_input_colmap()[:48], dtype=torch.long, device=w0.device)
+    valid = cm >= 0
+    parts = []
+    for w in (w0, w4):
+        wpe = torch.zeros((128, 48), dtype=torch.float32, device=w.device)
+        wpe[:, valid] = _f(w)[:, cm[valid]]
+        parts.append(pack_mma_b(wpe.t(), list(range(128)), 48))
+    packed = torch.cat(parts)
+    assert packed.numel() * 2 == 2 * 12288
+    return packed.contiguous()
+
+
 def head_input_colmap() -> List[int]:
     """Kernel colour-MLP input column -> reference column of [d'(3) | geo(15) | ones(14)]
     (fields/nersemble_nerfacto_field.py:371-377 + tcnn pad-with-1.0).  Kernel order:

@@ -352,6 +352,18 @@ class SE3DeformationField(nn.Module):
                                 positions=positions, sample_warp_codes=warp_code, want=("offsets",))
         return out["offsets"]
 
+    @torch.no_grad()
+    def offsets_vjp(self, positions: torch.Tensor, warp_code: torch.Tensor, cotangent: torch.Tensor,
+                    windows_param: Optional[float] = None) -> torch.Tensor:
+        """J^T . cotangent [n,3] for J = d compute_offsets / d positions (the WORLD positions passed in): how a cotangent
+        of the normalised offsets pulls back to the observed position (ops.deform_input_grad, divided by the box extent).
+        No autograd involved: nothing is recorded, and compute_offsets itself still refuses positions that require grad."""
+        d_pn = ops.deform_input_grad(self._native_params(), cotangent.reshape(-1, 3), window_deform=windows_param,
+                                     positions=positions.detach().reshape(-1, 3),
+                                     sample_warp_codes=warp_code.detach().reshape(-1, 128))
+        aabb = self.aabb.detach()
+        return d_pn / (aabb[1] - aabb[0]).to(d_pn.device)
+
     def _grad_params(self) -> List[nn.Parameter]:
         """Parameters in the order _DeformationFunction returns their gradients."""
         f = self.se3_field

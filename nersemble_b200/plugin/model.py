@@ -202,6 +202,8 @@ class NeRSembleNGPModel(Model):
                                          # samples, so the differentiable forward does not gather the tables a second time
         self.render_normals = False      # get_outputs / get_outputs_for_camera_ray_bundle also return "normals": world-space
                                          # surface normals composited with the render weights (unit vectors, [R,3] / [H,W,3])
+        self.render_normals_space = "canonical"  # "observation": the normals of the observed (deformed) surface, with the
+                                         # deformation Jacobian applied; "canonical": of the canonical surface the field stores
 
     def populate_modules(self):
         """models/nersemble_instant_ngp.py:81-179 (+ BaseModel.populate_modules, base.py:38-47)."""
@@ -341,19 +343,21 @@ class NeRSembleNGPModel(Model):
                                use_deformation=cfg.use_deformation_field, training=self.training, sampler="occupancy",
                                near_planes=near_planes, far_planes=far_planes, binaries=og.binaries, aabbs=og.aabbs,
                                step=cfg.render_step_size, cone_angle=cfg.cone_angle, uniform_time=uniform_time,
-                               line_gather=not self.frame_tables, want_normals=self.render_normals, **self._blend_opts())
+                               line_gather=not self.frame_tables, want_normals=self.render_normals,
+                               normals_space=self.render_normals_space, **self._blend_opts())
 
     @torch.no_grad()
     def _packed_normals(self, ray_bundle: RayBundle, ray_times, starts, ends, ray_indices, packed_info, weights, offsets,
                         line_gather: bool) -> Tensor:
         """Rendered normals [R,3] of packed samples the field already evaluated (the non-fused get_outputs paths):
-        world-space per-sample normals, composited with the render weights and normalised (ops.field_normals)."""
-        wh, _ = self._windows()
+        world-space per-sample normals in render_normals_space, composited with the render weights and normalised
+        (ops.field_normals)."""
+        wh, wd = self._windows()
         out = ops.field_normals(self.native_params(), window_hash=wh, offsets=offsets,
                                 origins=ray_bundle.origins.reshape(-1, 3), directions=ray_bundle.directions.reshape(-1, 3),
                                 ray_times=ray_times, t_starts=starts, t_ends=ends, ray_indices=ray_indices,
                                 line_gather=line_gather, world_space=True, packed_info=packed_info, weights=weights,
-                                **self._blend_opts())
+                                space=self.render_normals_space, window_deform=wd, **self._blend_opts())
         return out["ray_normals"]
 
     @torch.no_grad()

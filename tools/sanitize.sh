@@ -1,5 +1,6 @@
 #!/bin/bash
-# compute-sanitizer memcheck + racecheck (+ initcheck / synccheck) over every libnsb kernel (SURVEY 5: race detection).
+# compute-sanitizer memcheck + racecheck (+ initcheck / synccheck) over every libnsb kernel, deform_input_grad_kernel and
+# normals_observation_kernel included (SURVEY 5: race detection).
 # usage (on an H100 machine with compute-sanitizer): bash tools/sanitize.sh   -> $OUT/sanitize_*.txt, summary on stdout.
 set -u
 cd "$(dirname "$0")/.."

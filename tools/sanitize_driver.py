@@ -1,7 +1,8 @@
 """Small end-to-end exercise of every libnsb kernel, sized for compute-sanitizer (tools/sanitize.sh):
 fixed + occupancy march, visibility mask, fused field forward (inference and training instantiations, ragged last tile,
 several tiles per CTA so the mbarrier ring / tile counters wrap), composite fwd/bwd, losses, field / deformation
-backward, rank-1 expand + fused Adam, occupancy update, component kernels, surface normals."""
+backward, rank-1 expand + fused Adam, occupancy update, component kernels, surface normals (canonical and observation
+space), the deformation input gradient (ragged last tile, a device sample count below the buffer size)."""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
@@ -27,6 +28,13 @@ ops.field_normals(P, window_hash=20.25, positions=P.aabb[0].to(dev) + x * (P.aab
 for lg in (False, True):        # normals of the render's packed samples: timestep stack and line gather, per-ray composite
     ops.render_rays(P, o, d, t, window_hash=32.0, window_deform=7.0, sampler="fixed", n_per_ray=100, near_plane=bench.NEAR,
                     step=bench.STEP, line_gather=lg, want_normals=True)
+    ops.render_rays(P, o, d, t, window_hash=32.0, window_deform=7.0, sampler="fixed", n_per_ray=100, near_plane=bench.NEAR,
+                    step=bench.STEP, line_gather=lg, want_normals=True, normals_space="observation")
+ops.deform_input_grad(P, torch.randn((ts.shape[0] - 37, 3), device=dev), window_deform=3.3, origins=o, directions=d, ray_times=t,
+                      t_starts=ts[:-37], t_ends=te[:-37], ray_indices=ri[:-37],
+                      n_samples_dev=torch.tensor([9000], dtype=torch.int64, device=dev))
+ops.deform_input_grad(P, torch.randn((500, 3), device=dev), positions=P.aabb[0].to(dev) + x * (P.aabb[1] - P.aabb[0]).to(dev),
+                      sample_warp_codes=torch.randn((500, 128), device=dev) * 0.1)
 ops.field_forward(P, window_hash=32.0, window_deform=7.0, positions=P.aabb[0].to(dev) + x * (P.aabb[1] - P.aabb[0]).to(dev),
                   sample_times=torch.rand(500, device=dev), want=("sigma",))
 # plugin model: occupancy march + pre-pass + training step + occupancy update
