@@ -477,6 +477,34 @@ typedef struct {
 int nsb_normals_forward(const nsb_field_params *params, const nsb_field_opts *opts, const nsb_samples *samples,
                         const nsb_normals_args *args, void *stream);
 
+/* Isosurface of a density grid by marching tetrahedra (an extension: mesh export of one timestep; DESIGN 4.2d).
+ * Grid point (x, y, z), linear index x + nx * (y + ny * z), sits at box_min + (x, y, z) * h per axis and is INSIDE iff
+ * sigma > level.  Each cell is split into 6 tetrahedra (Kuhn split, one per axis permutation); every tetrahedron edge
+ * points in a non-negative direction and belongs to its lower grid point, which owns 7 edge slots in the order
+ * +x, +y, +z, +x+y, +x+z, +y+z, +x+y+z.  One vertex per edge whose ends differ in the inside test, at
+ * p0 + t (p1 - p0), t = (level - s0) / (s1 - s0), p0 the lower end; vertex ids follow (grid point, slot).  Faces follow
+ * (cell, tetrahedron, triangle), wound counter-clockwise seen from the outside (normal toward decreasing sigma).
+ * Two calls, no atomics (the output is the same bits on every run):
+ *   count: per-point crossing masks and per-tile sums, then their exclusive scan; the totals V, F land in
+ *          tile_sums[2 * n_tiles], tile_sums[2 * n_tiles + 1] (n_tiles = ceil(points / NSB_MESH_TILE)).
+ *   emit:  the caller passes the totals it read back; writes vertex_base, vertices [V][3] and faces [F][3]. */
+#define NSB_MESH_TILE 1024      /* grid points per CTA of the mesh passes */
+typedef struct {
+    const float *sigma;           /* [nz][ny][nx] density grid */
+    int64_t nx, ny, nz;           /* grid points per axis, each >= 2; nx * ny * nz < 2^31 */
+    float level;                  /* finite iso level */
+    float box_min[3];             /* world position of grid point (0, 0, 0) */
+    float h[3];                   /* grid spacing per axis */
+    uint8_t *point_mask;          /* [points] workspace: bits 0-6 crossing slots, bit 7 inside */
+    int32_t *vertex_base;         /* [points] workspace (emit): id of the point's first vertex */
+    int64_t *tile_sums;           /* [2 * n_tiles + 2] workspace: (vertices, faces) per tile, then the totals */
+    int64_t n_vertices, n_faces;  /* emit: the totals the count call left in tile_sums, each < 2^31 */
+    float *vertices;              /* emit: [n_vertices][3] out */
+    int32_t *faces;               /* emit: [n_faces][3] out */
+} nsb_mesh_args;
+int nsb_mesh_count(const nsb_mesh_args *args, void *stream);
+int nsb_mesh_emit(const nsb_mesh_args *args, void *stream);
+
 /* Training sampler WITHOUT host synchronisation (model_components/nersemble_volumetric_sampler.py:95-108 around nerfacc
  * OccGridEstimator.sampling): (1) nsb_march_occupancy_packed = count/scan/fill of nsb_march_occupancy as ONE cooperative
  * launch, the candidate count stays in the workspace header; (2) the caller evaluates the candidates' density with

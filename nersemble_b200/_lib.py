@@ -153,6 +153,16 @@ class DeformVjpArgs(C.Structure):   # nsb_deform_vjp_args
                 ("loss_scale", C.c_float), ("d_pn", C.c_void_p)]
 
 
+class MeshArgs(C.Structure):       # nsb_mesh_args
+    _fields_ = [("sigma", C.c_void_p), ("nx", C.c_int64), ("ny", C.c_int64), ("nz", C.c_int64), ("level", C.c_float),
+                ("box_min", C.c_float * 3), ("h", C.c_float * 3), ("point_mask", C.c_void_p), ("vertex_base", C.c_void_p),
+                ("tile_sums", C.c_void_p), ("n_vertices", C.c_int64), ("n_faces", C.c_int64), ("vertices", C.c_void_p),
+                ("faces", C.c_void_p)]
+
+
+MESH_TILE = 1024        # NSB_MESH_TILE
+
+
 class RenderWsHeader(C.Structure):
     _fields_ = [("barrier", C.c_uint32), ("depth_range", C.c_uint32 * 2), ("status", C.c_int32), ("n_total", C.c_int64),
                 ("reserved", C.c_int64 * 5)]
@@ -202,6 +212,8 @@ SYMBOLS = {
     "nsb_render_forward": (C.c_int, [C.POINTER(FieldParams), C.POINTER(FieldOpts), C.POINTER(RenderArgs), C.c_void_p]),
     "nsb_normals_forward": (C.c_int, [C.POINTER(FieldParams), C.POINTER(FieldOpts), C.POINTER(Samples),
                                       C.POINTER(NormalsArgs), C.c_void_p]),
+    "nsb_mesh_count": (C.c_int, [C.POINTER(MeshArgs), C.c_void_p]),
+    "nsb_mesh_emit": (C.c_int, [C.POINTER(MeshArgs), C.c_void_p]),
 }
 
 _lib = None

@@ -1091,6 +1091,167 @@ def render_rays(P: NativeParams, origins, directions, ray_times, *, window_hash=
     return out
 
 
+MESH_SPACES = ("observation", "canonical")
+MESH_SLAB_POINTS = 1 << 22          # grid points per field_forward call of the density pass
+MESH_FALLBACK_DIRECTION = (0.0, 0.0, -1.0)    # colour view direction of a vertex without a normal
+
+
+def mesh_grid(P: NativeParams, resolution, box=None):
+    """The grid of extract_mesh: (box_min [3], h [3], (nx, ny, nz)) as Python floats already rounded to float32.
+    box: [[x0, y0, z0], [x1, y1, z1]] (any nesting of 6 numbers), default the scene aabb.  An int `resolution` is the
+    number of points along the longest axis with cubic voxels, h = longest extent / (resolution - 1); the other axes get
+    round(extent / h) + 1 points (at least 2), so the grid ends within half a voxel of the box.  A 3-tuple (nx, ny, nz) is
+    taken as given, h = extent / (n - 1) per axis."""
+    import numpy as np
+    b = [float(v) for v in (P.aabb_list if box is None else torch.as_tensor(box, dtype=torch.float64).reshape(-1).tolist())]
+    if len(b) != 6:
+        raise ValueError(f"box must hold 6 numbers (min xyz, max xyz), got {len(b)}")
+    ext = [b[3 + k] - b[k] for k in range(3)]
+    if min(ext) <= 0:
+        raise ValueError(f"box must have a positive extent on every axis, got {ext}")
+    if isinstance(resolution, int):
+        if resolution < 2:
+            raise ValueError("resolution must be >= 2")
+        hh = max(ext) / (resolution - 1)
+        dims = tuple(max(2, int(round(e / hh)) + 1) for e in ext)
+        h = [hh] * 3
+    else:
+        dims = tuple(int(r) for r in resolution)
+        if len(dims) != 3 or min(dims) < 2:
+            raise ValueError(f"resolution must be an int or 3 ints, each >= 2, got {resolution!r}")
+        h = [ext[k] / (dims[k] - 1) for k in range(3)]
+    f32 = lambda v: float(np.float32(v))
+    return [f32(b[k]) for k in range(3)], [f32(v) for v in h], dims
+
+
+def density_grid(P: NativeParams, *, time: float, resolution, box=None, space: str = "observation", window_hash=None,
+                 window_deform=None, binaries: Optional[torch.Tensor] = None, aabbs: Optional[torch.Tensor] = None,
+                 disable_initial: bool = True, soft_transition: bool = True) -> Dict[str, object]:
+    """The density pass of extract_mesh: sigma [nz, ny, nx] (x fastest) of the grid of mesh_grid at one time.
+    Grid point (x, y, z) is at box_min + (x, y, z) * h, formed in float32 (product, then sum).  Density from field_forward
+    at `time` (its frame table): space="observation" through the deformation, "canonical" with use_deformation=False.
+    Positions are generated per z-slab of at most MESH_SLAB_POINTS points.  With binaries [levels, res, res, res] and
+    aabbs [levels, 6] (an OccGridEstimator's), sigma is 0 at points whose occupancy cell is empty, as the marcher skips
+    them: the first level whose box contains the point decides, points outside every level are empty.  The outermost
+    layer of grid points is set to 0, so every isosurface at a level >= 0 is closed.
+    Returns {"sigma", "box_min", "h"}."""
+    if space not in MESH_SPACES:
+        raise ValueError(f"space must be one of {MESH_SPACES}, got {space!r}")
+    if (binaries is None) != (aabbs is None):
+        raise ValueError("binaries and aabbs go together")
+    dev = P.tables.device
+    box_min, h, (nx, ny, nz) = mesh_grid(P, resolution, box)
+    if nx * ny * nz >= (1 << 31):
+        raise ValueError(f"the grid {nx} x {ny} x {nz} has 2^31 points or more")
+    sigma = torch.empty((nz, ny, nx), dtype=_F32, device=dev)
+    axis = [torch.arange(n, device=dev, dtype=_F32) * h[k] + box_min[k] for k, n in enumerate((nx, ny, nz))]
+    occ = None
+    if binaries is not None:
+        _need_cuda(binaries, aabbs)
+        occ = binaries.detach().to(torch.bool)
+        L, res = int(occ.shape[0]), int(occ.shape[1])
+        assert occ.shape[1:] == (res, res, res), "cubic occupancy grids only"
+        occ_ab = aabbs.detach().to(dev, _F32).reshape(L, 6)
+    slab = max(1, MESH_SLAB_POINTS // (nx * ny))
+    obs = space == "observation"
+    for z0 in range(0, nz, slab):
+        z1 = min(nz, z0 + slab)
+        Z, Y, X = torch.meshgrid(axis[2][z0:z1], axis[1], axis[0], indexing="ij")
+        pos = torch.stack([X, Y, Z], -1).reshape(-1, 3)
+        n = pos.shape[0]
+        s = field_forward(P, window_hash=window_hash, window_deform=window_deform, use_deformation=obs, positions=pos,
+                          sample_times=torch.full((n,), float(time), dtype=_F32, device=dev), uniform_time=float(time),
+                          want=("sigma",), disable_initial=disable_initial, soft_transition=soft_transition)["sigma"]
+        if occ is not None:
+            keep = torch.zeros((n,), dtype=torch.bool, device=dev)
+            seen = torch.zeros((n,), dtype=torch.bool, device=dev)
+            for l in range(L):        # the march's cell of a position: int(((p - aabb_min) / extent) * res)
+                lo, hi = occ_ab[l, :3], occ_ab[l, 3:]
+                u = (pos - lo) / (hi - lo)
+                inl = ((u >= 0) & (u < 1)).all(-1)
+                c = (u * res).long().clamp_(0, res - 1)
+                keep |= inl & ~seen & occ[l][c[:, 0], c[:, 1], c[:, 2]]
+                seen |= inl
+            s = torch.where(keep, s, torch.zeros_like(s))
+        sigma[z0:z1].view(-1).copy_(s)
+    for v in (sigma[0], sigma[-1], sigma[:, 0], sigma[:, -1], sigma[:, :, 0], sigma[:, :, -1]):
+        v.zero_()
+    return {"sigma": sigma, "box_min": box_min, "h": h}
+
+
+def marching_tetrahedra(sigma: torch.Tensor, level: float, box_min, h) -> Dict[str, torch.Tensor]:
+    """Isosurface {sigma = level} of a grid sigma [nz, ny, nx] (x fastest), grid point (x, y, z) at box_min + (x, y, z) * h
+    (nsb_mesh_count / nsb_mesh_emit): marching tetrahedra on the Kuhn split, inside = sigma > level.  Returns
+    {"vertices" [V,3] float32, "faces" [F,3] int32}: one vertex per crossing grid edge, ids in (grid point, edge slot)
+    order, faces in (cell, tetrahedron, triangle) order, counter-clockwise seen from outside (DESIGN 4.2d).  The same bits
+    on every run.  Reads the two totals back with ONE host synchronisation to allocate exact-size outputs: this is an
+    export, not a render path."""
+    _need_cuda(sigma)
+    if sigma.dim() != 3:
+        raise ValueError(f"sigma must be [nz, ny, nx], got {tuple(sigma.shape)}")
+    sg = _f32c(sigma)
+    nz, ny, nx = (int(v) for v in sg.shape)
+    dev = sg.device
+    a = _lib.MeshArgs()
+    a.sigma, a.nx, a.ny, a.nz, a.level = _ptr(sg), nx, ny, nz, float(level)
+    for k in range(3):
+        a.box_min[k], a.h[k] = float(box_min[k]), float(h[k])
+    lib = _lib.load()
+    n = nx * ny * nz
+    tiles = (n + _lib.MESH_TILE - 1) // _lib.MESH_TILE
+    point_mask = torch.empty((max(n, 1),), dtype=torch.uint8, device=dev)
+    vertex_base = torch.empty((max(n, 1),), dtype=torch.int32, device=dev)
+    tile_sums = torch.empty((2 * tiles + 2,), dtype=torch.int64, device=dev)
+    a.point_mask, a.vertex_base, a.tile_sums = _ptr(point_mask), _ptr(vertex_base), _ptr(tile_sums)
+    _lib.check(lib.nsb_mesh_count(C.byref(a), _stream()), "nsb_mesh_count")
+    V, F = tile_sums[2 * tiles:].tolist()           # the one host synchronisation: exact-size outputs
+    if V >= (1 << 31) or F >= (1 << 31):
+        raise RuntimeError(f"marching_tetrahedra: {V} vertices / {F} faces do not fit int32 ids; use a coarser grid")
+    out = {"vertices": torch.empty((V, 3), dtype=_F32, device=dev), "faces": torch.empty((F, 3), dtype=torch.int32, device=dev)}
+    a.n_vertices, a.n_faces = V, F
+    a.vertices, a.faces = _ptr(out["vertices"]), _ptr(out["faces"])
+    _lib.check(lib.nsb_mesh_emit(C.byref(a), _stream()), "nsb_mesh_emit")
+    return out
+
+
+def extract_mesh(P: NativeParams, *, time: float, level: float, resolution, box=None, space: str = "observation",
+                 window_hash=None, window_deform=None, binaries: Optional[torch.Tensor] = None,
+                 aabbs: Optional[torch.Tensor] = None, normals: bool = True, colours: bool = True,
+                 disable_initial: bool = True, soft_transition: bool = True) -> Dict[str, torch.Tensor]:
+    """Surface mesh of the density field at one time: density_grid, then marching_tetrahedra at `level` (>= 0), then
+    per-vertex normals and colours.  space="observation" is the observed (deformed) head of that frame, "canonical" the
+    surface the field stores.  Returns {"vertices" [V,3] float32 world, "faces" [F,3] int32, "normals" [V,3],
+    "colours" [V,3]} (normals / colours only when asked for).
+    normals: field_normals at the vertices in the same space, world space; zero where the warped position leaves the box.
+    colours: field_forward RGB seen head-on, view direction -normal (MESH_FALLBACK_DIRECTION where the normal is zero).
+    One host synchronisation (the mesh size); not differentiable."""
+    import math
+    if not math.isfinite(float(level)) or float(level) < 0:
+        raise ValueError(f"level must be finite and >= 0 (sigma is non-negative), got {level}")
+    g = density_grid(P, time=time, resolution=resolution, box=box, space=space, window_hash=window_hash,
+                     window_deform=window_deform, binaries=binaries, aabbs=aabbs, disable_initial=disable_initial,
+                     soft_transition=soft_transition)
+    out = marching_tetrahedra(g["sigma"], level, g["box_min"], g["h"])
+    del g
+    if not (normals or colours):
+        return out
+    v = out["vertices"]
+    V, dev = int(v.shape[0]), v.device
+    obs = space == "observation"
+    kw = dict(window_hash=window_hash, positions=v, sample_times=torch.full((V,), float(time), dtype=_F32, device=dev),
+              uniform_time=float(time), disable_initial=disable_initial, soft_transition=soft_transition)
+    off = field_forward(P, window_deform=window_deform, want=("offsets",), **kw)["offsets"] if obs else None
+    nrm = field_normals(P, offsets=off, world_space=True, space=space, window_deform=window_deform, **kw)["normals"]
+    if normals:
+        out["normals"] = nrm
+    if colours:
+        fb = torch.tensor(MESH_FALLBACK_DIRECTION, dtype=_F32, device=dev)
+        dirs = torch.where((nrm == 0).all(-1, keepdim=True), fb, -nrm)
+        out["colours"] = field_forward(P, window_deform=window_deform, use_deformation=obs, sample_directions=dirs,
+                                       want=("rgb",), **kw)["rgb"]
+    return out
+
+
 def render_packed(P: NativeParams, origins, directions, ray_times, t_starts, t_ends, ray_indices, packed_info, *,
                   window_hash=None, window_deform=None, use_deformation=True, training=False,
                   disable_initial=True, soft_transition=True) -> Dict[str, torch.Tensor]:

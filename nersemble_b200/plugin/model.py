@@ -2,7 +2,7 @@
 from __future__ import annotations
 
 from dataclasses import dataclass, field
-from math import sqrt
+from math import log, sqrt
 from typing import Dict, List, Optional, Tuple, Type
 
 import torch
@@ -10,6 +10,7 @@ from torch import Tensor, nn
 from torch.nn import Parameter, init
 
 from .. import ops
+from ..mesh import Mesh
 from ..nerfstudio_shim import (FieldHeadNames, Model, RayBundle, RaySamples, SceneBox, TrainingCallback,
                                TrainingCallbackAttributes, TrainingCallbackLocation)
 from .components import GenericScheduler, HashEnsembleConfig, SE3DeformationField, SE3DeformationFieldConfig
@@ -285,6 +286,29 @@ class NeRSembleNGPModel(Model):
     def _blend_opts(self):
         he = self.field.hash_ensemble
         return dict(disable_initial=he.disable_initial_hash_ensemble, soft_transition=he.use_soft_transition)
+
+    @torch.no_grad()
+    def extract_mesh(self, timestep: int, resolution=256, level: Optional[float] = None, space: str = "observation",
+                     respect_occupancy: bool = True, box=None) -> Mesh:
+        """Surface mesh of one timestep (ops.extract_mesh) with vertex normals and colours, at the current windows and
+        blend options.  level None: sigma = ln 2 / render_step_size, where one render step is half opaque.
+        space "observation": the head as the timestep's cameras saw it; "canonical": the surface the field stores (the
+        same without a deformation field).  respect_occupancy: cells the occupancy grid marks empty (e.g. after
+        plugin.occupancy_filter.filter_occupancy_grid) give no surface, as they give no samples in a render.
+        resolution / box as in ops.mesh_grid (default box: the scene box)."""
+        cfg = self.config
+        if not 0 <= int(timestep) < cfg.n_timesteps:
+            raise ValueError(f"timestep must be in [0, {cfg.n_timesteps}), got {timestep}")
+        if level is None:
+            level = log(2.0) / cfg.render_step_size
+        wh, wd = self._windows()
+        og = self.occupancy_grid
+        out = ops.extract_mesh(self.native_params(), time=int(timestep) / max(cfg.n_timesteps - 1, 1), level=level,
+                               resolution=resolution, box=box,
+                               space=space if cfg.use_deformation_field else "canonical", window_hash=wh, window_deform=wd,
+                               binaries=og.binaries if respect_occupancy else None,
+                               aabbs=og.aabbs if respect_occupancy else None, **self._blend_opts())
+        return Mesh.from_tensors(out)
 
     # ------------------------------------------------------------------ callbacks
     def get_training_callbacks(self, training_callback_attributes: TrainingCallbackAttributes) -> List[TrainingCallback]:

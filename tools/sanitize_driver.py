@@ -2,7 +2,8 @@
 fixed + occupancy march, visibility mask, fused field forward (inference and training instantiations, ragged last tile,
 several tiles per CTA so the mbarrier ring / tile counters wrap), composite fwd/bwd, losses, field / deformation
 backward, rank-1 expand + fused Adam, occupancy update, component kernels, surface normals (canonical and observation
-space), the deformation input gradient (ragged last tile, a device sample count below the buffer size)."""
+space), the deformation input gradient (ragged last tile, a device sample count below the buffer size), the mesh export
+(a ragged last tile of grid points, an occupancy grid, vertex normals and colours)."""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
@@ -37,6 +38,8 @@ ops.deform_input_grad(P, torch.randn((500, 3), device=dev), positions=P.aabb[0].
                       sample_warp_codes=torch.randn((500, 128), device=dev) * 0.1)
 ops.field_forward(P, window_hash=32.0, window_deform=7.0, positions=P.aabb[0].to(dev) + x * (P.aabb[1] - P.aabb[0]).to(dev),
                   sample_times=torch.rand(500, device=dev), want=("sigma",))
+ops.extract_mesh(P, time=0.5, level=0.5, resolution=(13, 11, 9), window_hash=32.0, window_deform=7.0,
+                 binaries=torch.rand((1, 16, 16, 16), device=dev) > 0.3, aabbs=P.aabb.reshape(1, 6).to(dev))
 # plugin model: occupancy march + pre-pass + training step + occupancy update
 m = bench.build_model(S, dev).train()
 occ = bench.blob_occupancy(seed=5)
