@@ -29,6 +29,8 @@
  *                          for the stand-alone field and deformation modules of the component API)
  *   nsb_deform_input_grad  torch.autograd.grad of SE3DeformationField.compute_offsets with respect to its input
  *                          positions (an extension: the reference never differentiates the warp by position)
+ *   nsb_deform_jacobian / nsb_deform_inverse
+ *                          the warp's Jacobian and its inverse (an extension: point tracking across timesteps)
  *   nsb_table_adam_step    torch.optim.Adam on the 8 tcnn grid tensors (scripts/train/train_nersemble.py:243-247) and
  *                          tcnn's per-call fp32 -> fp16 cast of the table parameters
  */
@@ -293,6 +295,47 @@ typedef struct {
 } nsb_deform_vjp_args;
 int nsb_deform_input_grad(const nsb_field_params *params, const nsb_field_opts *opts, const nsb_samples *samples,
                           const nsb_deform_vjp_args *args, void *stream);
+
+/* Jacobian and inverse of the deformation (an extension: point tracking across timesteps; DESIGN 4.2e).  Samples are
+ * positions-based (samples->positions, sample_times rounded like every kernel, or per-sample warp codes as
+ * samples->sample_code_bias); the warp codes enter as in nsb_deform_input_grad.  Both run the stem in forward mode: per
+ * point one primal row (the field kernels' operand rounding) and three tangent rows (d / d p_n[k], fp16 MMA operands
+ * scaled by tangent_scale and divided back at the heads), 32 points per 128-row tile.  No atomics: bit-identical from
+ * run to run.  Samples beyond *n_samples_dev (when given) are not touched.  Not differentiable.
+ *
+ * nsb_deform_jacobian: offsets [n][3], the normalised offsets nsb_field_forward writes (equal up to the fp16 operand
+ * rounding of its deformation role), and J [n][3][3], J[i][k] = d offset_i / d p_n[k] (the J of nsb_deform_input_grad).
+ * A row whose warp is NaN (the identity in the forward) gets J = 0. */
+typedef struct {
+    float tangent_scale;      /* > 0: factor on the tangent rows' fp16 operands (python: ops.JVP_TANGENT_SCALE) */
+    float *offsets;           /* [n][3] out */
+    float *jacobian;          /* [n][3][3] out */
+} nsb_deform_jac_args;
+int nsb_deform_jacobian(const nsb_field_params *params, const nsb_field_opts *opts, const nsb_samples *samples,
+                        const nsb_deform_jac_args *args, void *stream);
+
+/* nsb_deform_inverse: for each target c = samples->positions[i] (a world position of the warped hash input, i.e. an
+ * observed position plus its normalised offset, as the field kernels form it), the observed position p whose warp lands
+ * on c at the sample's time: the root of F(p_n) = p_n + D^-1 offset(p_n) - c_n, D = diag(aabb extent), by damped Newton.
+ * Each iteration evaluates F and J at every point's trial; a trial with |F|inf below the best so far becomes the best and
+ * the next trial is best - (I + D^-1 J)^-1 F (fp32 3 x 3 solve; |det| <= 1e-6 stops the point as singular), any other
+ * trial is replaced by the midpoint of the best and the trial.  A point stops when its best |F|inf < tol (converged), after
+ * max_iter new trials (not converged) or at a singular system.  A 32-point tile iterates until all of its points stop. */
+#define NSB_INV_CONVERGED 0
+#define NSB_INV_NOT_CONVERGED 1
+#define NSB_INV_SINGULAR 2
+typedef struct {
+    float tangent_scale;      /* as in nsb_deform_jac_args */
+    const float *init;        /* [n][3] world initial guesses, or NULL: the targets */
+    int32_t max_iter;         /* 1..64 */
+    float tol;                /* finite, > 0: on |F|inf in normalised units */
+    float *positions;         /* [n][3] out: the best position (world); the initial guess bit for bit if it converged */
+    float *residual;          /* [n] out: |F|inf at that position, from the kernel's own evaluation */
+    int32_t *iterations;      /* [n] out: trials evaluated after the initial guess */
+    int32_t *status;          /* [n] out: NSB_INV_CONVERGED / NSB_INV_NOT_CONVERGED / NSB_INV_SINGULAR */
+} nsb_deform_inv_args;
+int nsb_deform_inverse(const nsb_field_params *params, const nsb_field_opts *opts, const nsb_samples *samples,
+                       const nsb_deform_inv_args *args, void *stream);
 
 /* Fused hash-table optimiser step.  Replaces, for the table parameter only, what the reference's training loop does
  * with torch: materialise the dense fp32 gradient of the 8 tcnn grids, run torch.optim.Adam over it (nerfstudio

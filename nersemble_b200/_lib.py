@@ -153,6 +153,18 @@ class DeformVjpArgs(C.Structure):   # nsb_deform_vjp_args
                 ("loss_scale", C.c_float), ("d_pn", C.c_void_p)]
 
 
+class DeformJacArgs(C.Structure):   # nsb_deform_jac_args
+    _fields_ = [("tangent_scale", C.c_float), ("offsets", C.c_void_p), ("jacobian", C.c_void_p)]
+
+
+class DeformInvArgs(C.Structure):   # nsb_deform_inv_args
+    _fields_ = [("tangent_scale", C.c_float), ("init", C.c_void_p), ("max_iter", C.c_int32), ("tol", C.c_float),
+                ("positions", C.c_void_p), ("residual", C.c_void_p), ("iterations", C.c_void_p), ("status", C.c_void_p)]
+
+
+INV_CONVERGED, INV_NOT_CONVERGED, INV_SINGULAR = 0, 1, 2     # NSB_INV_*
+
+
 class MeshArgs(C.Structure):       # nsb_mesh_args
     _fields_ = [("sigma", C.c_void_p), ("nx", C.c_int64), ("ny", C.c_int64), ("nz", C.c_int64), ("level", C.c_float),
                 ("box_min", C.c_float * 3), ("h", C.c_float * 3), ("point_mask", C.c_void_p), ("vertex_base", C.c_void_p),
@@ -186,6 +198,10 @@ SYMBOLS = {
                                       C.POINTER(DeformBwdArgs), C.c_void_p]),
     "nsb_deform_input_grad": (C.c_int, [C.POINTER(FieldParams), C.POINTER(FieldOpts), C.POINTER(Samples),
                                         C.POINTER(DeformVjpArgs), C.c_void_p]),
+    "nsb_deform_jacobian": (C.c_int, [C.POINTER(FieldParams), C.POINTER(FieldOpts), C.POINTER(Samples),
+                                      C.POINTER(DeformJacArgs), C.c_void_p]),
+    "nsb_deform_inverse": (C.c_int, [C.POINTER(FieldParams), C.POINTER(FieldOpts), C.POINTER(Samples),
+                                     C.POINTER(DeformInvArgs), C.c_void_p]),
     "nsb_losses_forward": (C.c_int, [C.POINTER(LossArgs), C.c_void_p]),
     "nsb_losses_backward": (C.c_int, [C.POINTER(LossArgs), C.c_void_p]),
     "nsb_table_adam_step": (C.c_int, [C.POINTER(TableAdamArgs), C.c_void_p]),

@@ -1,8 +1,9 @@
-"""Triangle-mesh result of NeRSembleNGPModel.extract_mesh / ops.extract_mesh and its PLY export (numpy only)."""
+"""Triangle-mesh results of NeRSembleNGPModel.extract_mesh / extract_mesh_sequence (ops.extract_mesh /
+ops.extract_mesh_sequence) and their PLY export (numpy only)."""
 from __future__ import annotations
 
 from dataclasses import dataclass
-from typing import Optional
+from typing import List, Optional, Sequence
 
 import numpy as np
 
@@ -80,3 +81,46 @@ class Mesh:
         rgb = stack(("red", "green", "blue"), np.float32)
         return Mesh(stack("xyz", np.float32), np.ascontiguousarray(face["v"], dtype=np.int32),
                     stack(("nx", "ny", "nz"), np.float32), None if rgb is None else rgb / 255.0)
+
+
+@dataclass
+class MeshSequence:
+    """One connectivity for every frame: the reference frame's mesh with its vertices tracked along the deformation
+    field.  converged[i, v] says whether vertex v's track to frame i converged; sigma[i, v] is the density at the tracked
+    vertex (near the extraction level where the deformation alone moved the surface, away from it where the hash
+    ensemble's blend moved it)."""
+    faces: np.ndarray                       # int32 [F, 3], shared by every frame
+    vertices: np.ndarray                    # float32 [K, V, 3], world space
+    timesteps: List[int]                    # the frames' timesteps
+    converged: np.ndarray                   # bool [K, V]
+    sigma: np.ndarray                       # float32 [K, V]
+    normals: Optional[np.ndarray] = None    # float32 [K, V, 3]
+    colours: Optional[np.ndarray] = None    # float32 [K, V, 3]
+
+    @staticmethod
+    def from_tensors(out: dict, timesteps: Sequence[int]) -> "MeshSequence":
+        """From the dict of ops.extract_mesh_sequence (device tensors)."""
+        get = lambda k, dt: None if out.get(k) is None else out[k].detach().cpu().numpy().astype(dt)
+        return MeshSequence(get("faces", np.int32), get("vertices", np.float32), [int(t) for t in timesteps],
+                            get("converged", bool), get("sigma", np.float32), get("normals", np.float32),
+                            get("colours", np.float32))
+
+    def __len__(self) -> int:
+        return len(self.timesteps)
+
+    def frame(self, i: int) -> Mesh:
+        """Frame i (index into timesteps) as a Mesh."""
+        pick = lambda a: None if a is None else a[i]
+        return Mesh(self.vertices[i], self.faces, pick(self.normals), pick(self.colours))
+
+    def save_ply(self, pattern: str) -> List[str]:
+        """One PLY per frame through Mesh.save_ply; pattern.format(timestep) names each file (e.g. "head_{:03d}.ply").
+        Returns the paths."""
+        paths = []
+        for i, t in enumerate(self.timesteps):
+            path = pattern.format(t)
+            if path in paths:
+                raise ValueError(f"the pattern {pattern!r} gives the same file for two frames")
+            self.frame(i).save_ply(path)
+            paths.append(path)
+        return paths

@@ -365,6 +365,125 @@ def deform_input_grad(P: NativeParams, u: torch.Tensor, *, window_deform=None, l
     return out
 
 
+# Scale of the fp16 tangent rows of the deformation Jacobian (nsb_deform_jacobian / nsb_deform_inverse).  The largest
+# posenc tangent is window * 2 pi 2^6 = 402 per unit of p_n; scaled by 1/16 it is 25, so the stem's tangent rows stay three
+# orders of magnitude below fp16's maximum (65504) while the entries that matter stay far above its smallest normal (6.1e-5).
+JVP_TANGENT_SCALE = 1.0 / 16.0
+INVERSE_MAX_ITER = 64
+
+
+def _positions_samples(sample_kw, who: str):
+    if any(sample_kw.get(k) is not None for k in ("origins", "directions", "t_starts", "t_ends", "ray_indices", "ray_times")):
+        raise ValueError(f"{who}: positions-based samples only (positions, sample_times)")
+    if sample_kw.get("positions") is None:
+        raise ValueError(f"{who}: positions are required")
+
+
+def deform_jacobian(P: NativeParams, *, window_deform=None, sample_warp_codes: Optional[torch.Tensor] = None,
+                    n_samples_dev: Optional[torch.Tensor] = None, **sample_kw) -> Dict[str, torch.Tensor]:
+    """Offsets and Jacobian of the SE(3) deformation at given points (nsb_deform_jacobian), in one forward-mode pass:
+    {"offsets" [n,3]: the normalised offsets field_forward(want=("offsets",)) reports (equal up to fp16 operand rounding),
+     "jacobian" [n,3,3]: J[i][k] = d offset_i / d p_n[k], p_n the normalised position -- the J whose transpose
+     deform_input_grad applies}.  Samples: positions [n,3] with sample_times [n] (table warp codes of the rounded
+    timestep) or sample_warp_codes [n,128].  Not differentiable."""
+    _positions_samples(sample_kw, "deform_jacobian")
+    keep: list = []
+    s = _lib.Samples()
+    n = _fill_samples(s, keep, **sample_kw)
+    dev = sample_kw["positions"].device
+    if sample_warp_codes is not None:
+        _fill_sample_code_bias(P, s, keep, sample_warp_codes, n, dev)
+    if n_samples_dev is not None:
+        assert n_samples_dev.dtype == torch.int64 and n_samples_dev.is_cuda and n_samples_dev.numel() == 1
+        s.n_samples_dev = _ptr(n_samples_dev); keep.append(n_samples_dev)
+    out = {"offsets": torch.empty((n, 3), dtype=_F32, device=dev), "jacobian": torch.empty((n, 3, 3), dtype=_F32, device=dev)}
+    if n == 0:
+        return out
+    a = _lib.DeformJacArgs()
+    a.tangent_scale, a.offsets, a.jacobian = JVP_TANGENT_SCALE, _ptr(out["offsets"]), _ptr(out["jacobian"])
+    opts = make_opts(None, window_deform, True, False)
+    cp = P.c_params()
+    _lib.check(_lib.load().nsb_deform_jacobian(C.byref(cp), C.byref(opts), C.byref(s), C.byref(a), _stream()),
+               "nsb_deform_jacobian")
+    return out
+
+
+def _check_newton(max_iter, tol, who: str):
+    import math
+    if not isinstance(max_iter, int) or not 1 <= max_iter <= INVERSE_MAX_ITER:
+        raise ValueError(f"{who}: max_iter must be an int in 1..{INVERSE_MAX_ITER}, got {max_iter!r}")
+    if not (math.isfinite(float(tol)) and float(tol) > 0):
+        raise ValueError(f"{who}: tol must be finite and > 0, got {tol!r}")
+
+
+def deform_inverse(P: NativeParams, targets: torch.Tensor, *, sample_times: Optional[torch.Tensor] = None,
+                   uniform_time: Optional[float] = None, init: Optional[torch.Tensor] = None, window_deform=None,
+                   sample_warp_codes: Optional[torch.Tensor] = None, max_iter: int = 20, tol: float = 1e-4) -> Dict[str, torch.Tensor]:
+    """Inverse of the deformation (nsb_deform_inverse): for each target c [n,3] -- a world position of the warped hash
+    input, i.e. an observed position plus its normalised offset, as the field kernels form it -- the observed position p
+    whose warp at the given time lands on c: the root of p_n + D^-1 offset(p_n) - c_n by damped Newton in the kernel.
+    Time per point (sample_times [n]) or for all (uniform_time), or per-point warp codes (sample_warp_codes [n,128]).
+    init [n,3]: initial guesses (default: the targets).  tol: on |F|inf in normalised units (1e-4 is about 1/20 of a voxel
+    of a 512^3 grid).  Returns {"positions" [n,3] world (the best trial; the initial guess bit for bit when it already
+    converged), "residual" [n] (|F|inf there), "iterations" [n] int32, "converged" [n] bool, "status" [n] int32
+    (_lib.INV_CONVERGED / INV_NOT_CONVERGED / INV_SINGULAR)}.  Not differentiable."""
+    _check_newton(max_iter, tol, "deform_inverse")
+    if (sample_times is not None) + (uniform_time is not None) + (sample_warp_codes is not None) > 1:
+        raise ValueError("deform_inverse: give one of sample_times, uniform_time, sample_warp_codes")
+    targets = _f32c(targets).reshape(-1, 3)
+    _need_cuda(targets)
+    n, dev = int(targets.shape[0]), targets.device
+    if uniform_time is not None:
+        sample_times = torch.full((n,), float(uniform_time), dtype=_F32, device=dev)
+    keep: list = []
+    s = _lib.Samples()
+    _fill_samples(s, keep, positions=targets, sample_times=sample_times)
+    if sample_warp_codes is not None:
+        _fill_sample_code_bias(P, s, keep, sample_warp_codes, n, dev)
+    a = _lib.DeformInvArgs()
+    if init is not None:
+        init = _f32c(init).reshape(-1, 3)
+        _need_cuda(init)
+        assert init.shape[0] == n, (init.shape, n)
+        a.init = _ptr(init); keep.append(init)
+    out = {"positions": torch.empty((n, 3), dtype=_F32, device=dev), "residual": torch.empty((n,), dtype=_F32, device=dev),
+           "iterations": torch.empty((n,), dtype=torch.int32, device=dev), "status": torch.empty((n,), dtype=torch.int32, device=dev)}
+    if n > 0:
+        a.tangent_scale, a.max_iter, a.tol = JVP_TANGENT_SCALE, int(max_iter), float(tol)
+        a.positions, a.residual = _ptr(out["positions"]), _ptr(out["residual"])
+        a.iterations, a.status = _ptr(out["iterations"]), _ptr(out["status"])
+        opts = make_opts(None, window_deform, True, False)
+        cp = P.c_params()
+        _lib.check(_lib.load().nsb_deform_inverse(C.byref(cp), C.byref(opts), C.byref(s), C.byref(a), _stream()),
+                   "nsb_deform_inverse")
+    out["converged"] = out["status"] == _lib.INV_CONVERGED
+    return out
+
+
+def track_points(P: NativeParams, points: torch.Tensor, *, time_from: float, times_to: Sequence[float], window_deform=None,
+                 max_iter: int = 20, tol: float = 1e-4) -> Dict[str, torch.Tensor]:
+    """Follow observed points of the frame at `time_from` to the frames at `times_to` along the deformation field: the
+    canonical target is c = p + offset(p) from deform_jacobian's own forward at time_from, then deform_inverse at each
+    time with init = points.  Tracking to time_from itself returns the points bit for bit with 0 iterations.  Returns
+    {"positions" [K,n,3], "residual" [K,n], "iterations" [K,n], "converged" [K,n]} for the K times.  A track follows the
+    deformation's motion only: where the hash ensemble's blend moved the surface between frames, a tracked surface point
+    sits off that frame's isosurface."""
+    _check_newton(max_iter, tol, "track_points")
+    points = _f32c(points).reshape(-1, 3)
+    _need_cuda(points)
+    n, dev = int(points.shape[0]), points.device
+    off = deform_jacobian(P, window_deform=window_deform, positions=points,
+                          sample_times=torch.full((n,), float(time_from), dtype=_F32, device=dev))["offsets"]
+    targets = points + off
+    res = [deform_inverse(P, targets, uniform_time=float(t), init=points, window_deform=window_deform, max_iter=max_iter,
+                          tol=tol) for t in times_to]
+    if not res:
+        return {"positions": torch.empty((0, n, 3), dtype=_F32, device=dev), "residual": torch.empty((0, n), dtype=_F32, device=dev),
+                "iterations": torch.empty((0, n), dtype=torch.int32, device=dev),
+                "converged": torch.empty((0, n), dtype=torch.bool, device=dev)}
+    return {k: torch.stack([r[k] for r in res]) for k in ("positions", "residual", "iterations", "converged")}
+
+
 def _world_grad_scale(P: NativeParams):
     """Per-axis factor that turns d h0 / d(normalised position) into d h0 / d(world position): 1 / aabb extent."""
     a = P.aabb_list
@@ -1233,22 +1352,74 @@ def extract_mesh(P: NativeParams, *, time: float, level: float, resolution, box=
                      soft_transition=soft_transition)
     out = marching_tetrahedra(g["sigma"], level, g["box_min"], g["h"])
     del g
-    if not (normals or colours):
+    out.update(vertex_attributes(P, out["vertices"], time=time, space=space, normals=normals, colours=colours,
+                                 window_hash=window_hash, window_deform=window_deform, disable_initial=disable_initial,
+                                 soft_transition=soft_transition))
+    return out
+
+
+def vertex_attributes(P: NativeParams, vertices: torch.Tensor, *, time: float, space: str = "observation",
+                      normals: bool = True, colours: bool = True, sigma: bool = False, window_hash=None, window_deform=None,
+                      disable_initial: bool = True, soft_transition: bool = True) -> Dict[str, torch.Tensor]:
+    """The per-vertex attributes of extract_mesh at world `vertices` [V,3] and one time: "normals" (field_normals in
+    `space`, world space, zero where the warped position leaves the box), "colours" (field_forward RGB seen head-on, view
+    direction -normal, MESH_FALLBACK_DIRECTION where the normal is zero) and "sigma" (the density there), each when asked
+    for."""
+    out: Dict[str, torch.Tensor] = {}
+    if not (normals or colours or sigma):
         return out
-    v = out["vertices"]
+    v = vertices
     V, dev = int(v.shape[0]), v.device
     obs = space == "observation"
     kw = dict(window_hash=window_hash, positions=v, sample_times=torch.full((V,), float(time), dtype=_F32, device=dev),
               uniform_time=float(time), disable_initial=disable_initial, soft_transition=soft_transition)
-    off = field_forward(P, window_deform=window_deform, want=("offsets",), **kw)["offsets"] if obs else None
-    nrm = field_normals(P, offsets=off, world_space=True, space=space, window_deform=window_deform, **kw)["normals"]
-    if normals:
-        out["normals"] = nrm
+    if normals or colours:
+        off = field_forward(P, window_deform=window_deform, want=("offsets",), **kw)["offsets"] if obs else None
+        nrm = field_normals(P, offsets=off, world_space=True, space=space, window_deform=window_deform, **kw)["normals"]
+        if normals:
+            out["normals"] = nrm
     if colours:
         fb = torch.tensor(MESH_FALLBACK_DIRECTION, dtype=_F32, device=dev)
         dirs = torch.where((nrm == 0).all(-1, keepdim=True), fb, -nrm)
         out["colours"] = field_forward(P, window_deform=window_deform, use_deformation=obs, sample_directions=dirs,
                                        want=("rgb",), **kw)["rgb"]
+    if sigma:
+        out["sigma"] = field_forward(P, window_deform=window_deform, use_deformation=obs, want=("sigma",), **kw)["sigma"]
+    return out
+
+
+def extract_mesh_sequence(P: NativeParams, *, times: Sequence[float], reference_time: float, level: float, resolution,
+                          box=None, space: str = "observation", window_hash=None, window_deform=None,
+                          binaries: Optional[torch.Tensor] = None, aabbs: Optional[torch.Tensor] = None,
+                          normals: bool = True, colours: bool = True, disable_initial: bool = True,
+                          soft_transition: bool = True, max_iter: int = 20, tol: float = 1e-4) -> Dict[str, object]:
+    """A mesh sequence with one connectivity: extract_mesh's mesh of the frame at `reference_time` (no attributes), its
+    vertices tracked to every time in `times` (track_points; space="observation"), and per frame the vertex attributes of
+    extract_mesh at the tracked vertices plus sigma there.  space="canonical" (or a field without deformation, when the
+    caller passes it) keeps the reference mesh's vertices in every frame.  Returns {"faces" [F,3], "vertices" [K,V,3],
+    "converged" [K,V], "residual" [K,V], "sigma" [K,V], "normals" / "colours" [K,V,3] (when asked for)}."""
+    _check_newton(max_iter, tol, "extract_mesh_sequence")
+    ref = extract_mesh(P, time=reference_time, level=level, resolution=resolution, box=box, space=space,
+                       window_hash=window_hash, window_deform=window_deform, binaries=binaries, aabbs=aabbs, normals=False,
+                       colours=False, disable_initial=disable_initial, soft_transition=soft_transition)
+    v0 = ref["vertices"]
+    V, dev = int(v0.shape[0]), v0.device
+    times = [float(t) for t in times]
+    if space == "observation" and V > 0:
+        tr = track_points(P, v0, time_from=float(reference_time), times_to=times, window_deform=window_deform,
+                          max_iter=max_iter, tol=tol)
+    else:
+        K = len(times)
+        tr = {"positions": v0.unsqueeze(0).expand(K, V, 3).contiguous(), "residual": torch.zeros((K, V), dtype=_F32, device=dev),
+              "converged": torch.ones((K, V), dtype=torch.bool, device=dev)}
+    out: Dict[str, object] = {"faces": ref["faces"], "vertices": tr["positions"], "converged": tr["converged"],
+                              "residual": tr["residual"]}
+    per = [vertex_attributes(P, tr["positions"][i], time=t, space=space, normals=normals, colours=colours, sigma=True,
+                             window_hash=window_hash, window_deform=window_deform, disable_initial=disable_initial,
+                             soft_transition=soft_transition) for i, t in enumerate(times)]
+    for k in ("sigma", "normals", "colours"):
+        if per and k in per[0]:
+            out[k] = torch.stack([p[k] for p in per])
     return out
 
 

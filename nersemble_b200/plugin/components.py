@@ -364,6 +364,29 @@ class SE3DeformationField(nn.Module):
         aabb = self.aabb.detach()
         return d_pn / (aabb[1] - aabb[0]).to(d_pn.device)
 
+    @torch.no_grad()
+    def offsets_jacobian(self, positions: torch.Tensor, warp_code: torch.Tensor,
+                         windows_param: Optional[float] = None) -> Dict[str, torch.Tensor]:
+        """{"offsets" [n,3]: compute_offsets' values (equal up to fp16 operand rounding), "jacobian" [n,3,3]:
+        d compute_offsets_i / d positions_k for the WORLD positions passed in} in one forward-mode pass
+        (ops.deform_jacobian, whose normalised-position Jacobian is divided by the box extent per column).  No autograd."""
+        out = ops.deform_jacobian(self._native_params(), window_deform=windows_param,
+                                  positions=positions.detach().reshape(-1, 3),
+                                  sample_warp_codes=warp_code.detach().reshape(-1, 128))
+        aabb = self.aabb.detach()
+        out["jacobian"] = out["jacobian"] / (aabb[1] - aabb[0]).to(out["jacobian"].device)
+        return out
+
+    @torch.no_grad()
+    def inverse(self, canonical_positions: torch.Tensor, warp_code: torch.Tensor, windows_param: Optional[float] = None,
+                init: Optional[torch.Tensor] = None, max_iter: int = 20, tol: float = 1e-4) -> Dict[str, torch.Tensor]:
+        """The positions p with p + compute_offsets(p, warp_code) = canonical_positions (world; the normalised offset added
+        to the world position, as the field does), by damped Newton in the kernel (ops.deform_inverse): {"positions",
+        "residual", "iterations", "converged", "status"}.  tol is on the residual in normalised units.  No autograd."""
+        return ops.deform_inverse(self._native_params(), canonical_positions.detach().reshape(-1, 3), init=init,
+                                  window_deform=windows_param, sample_warp_codes=warp_code.detach().reshape(-1, 128),
+                                  max_iter=max_iter, tol=tol)
+
     def _grad_params(self) -> List[nn.Parameter]:
         """Parameters in the order _DeformationFunction returns their gradients."""
         f = self.se3_field

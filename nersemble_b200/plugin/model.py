@@ -10,7 +10,7 @@ from torch import Tensor, nn
 from torch.nn import Parameter, init
 
 from .. import ops
-from ..mesh import Mesh
+from ..mesh import Mesh, MeshSequence
 from ..nerfstudio_shim import (FieldHeadNames, Model, RayBundle, RaySamples, SceneBox, TrainingCallback,
                                TrainingCallbackAttributes, TrainingCallbackLocation)
 from .components import GenericScheduler, HashEnsembleConfig, SE3DeformationField, SE3DeformationFieldConfig
@@ -309,6 +309,56 @@ class NeRSembleNGPModel(Model):
                                binaries=og.binaries if respect_occupancy else None,
                                aabbs=og.aabbs if respect_occupancy else None, **self._blend_opts())
         return Mesh.from_tensors(out)
+
+    def _timestep_time(self, timestep: int) -> float:
+        n = self.config.n_timesteps
+        if not 0 <= int(timestep) < n:
+            raise ValueError(f"timestep must be in [0, {n}), got {timestep}")
+        return int(timestep) / max(n - 1, 1)
+
+    @torch.no_grad()
+    def track_points(self, points: Tensor, timestep_from: int, timesteps_to, max_iter: int = 20,
+                     tol: float = 1e-4) -> Dict[str, Tensor]:
+        """Follow observed world points [n,3] of frame `timestep_from` to the frames `timesteps_to` along the deformation
+        field (ops.track_points) at the current deformation window: {"positions" [K,n,3], "residual" [K,n] (|F|inf in
+        normalised units), "converged" [K,n]}.  A track follows the deformation's motion, not the hash ensemble's: see
+        DESIGN 4.2e.  Without a deformation field every frame is the same space: the points come back unchanged and
+        nothing is launched."""
+        t_from = self._timestep_time(timestep_from)
+        t_to = [self._timestep_time(t) for t in timesteps_to]
+        pts = points.detach().float().reshape(-1, 3)
+        if self.deformation_field is None or not self.config.use_deformation_field:
+            K, n = len(t_to), pts.shape[0]
+            return {"positions": pts.unsqueeze(0).expand(K, n, 3).clone(),
+                    "residual": torch.zeros((K, n), dtype=torch.float32, device=pts.device),
+                    "converged": torch.ones((K, n), dtype=torch.bool, device=pts.device)}
+        _, wd = self._windows()
+        out = ops.track_points(self.native_params(), pts.to(self.scene_aabb.device), time_from=t_from, times_to=t_to,
+                               window_deform=wd, max_iter=max_iter, tol=tol)
+        return {k: out[k] for k in ("positions", "residual", "converged")}
+
+    @torch.no_grad()
+    def extract_mesh_sequence(self, timesteps, reference_timestep: int, resolution=256, level: Optional[float] = None,
+                              space: str = "observation", respect_occupancy: bool = True, box=None, normals: bool = True,
+                              colours: bool = True) -> MeshSequence:
+        """A mesh sequence with one connectivity (ops.extract_mesh_sequence): extract_mesh of `reference_timestep` (same
+        level, grid, occupancy and windows), its vertices tracked to every timestep in `timesteps`, and per frame vertex
+        normals, colours and sigma at the tracked vertices.  space "canonical", or a model without a deformation field,
+        keeps the reference vertices in every frame."""
+        cfg = self.config
+        t_ref = self._timestep_time(reference_timestep)
+        times = [self._timestep_time(t) for t in timesteps]
+        if level is None:
+            level = log(2.0) / cfg.render_step_size
+        wh, wd = self._windows()
+        og = self.occupancy_grid
+        out = ops.extract_mesh_sequence(self.native_params(), times=times, reference_time=t_ref, level=level,
+                                        resolution=resolution, box=box,
+                                        space=space if cfg.use_deformation_field else "canonical", window_hash=wh,
+                                        window_deform=wd, binaries=og.binaries if respect_occupancy else None,
+                                        aabbs=og.aabbs if respect_occupancy else None, normals=normals, colours=colours,
+                                        **self._blend_opts())
+        return MeshSequence.from_tensors(out, [int(t) for t in timesteps])
 
     # ------------------------------------------------------------------ callbacks
     def get_training_callbacks(self, training_callback_attributes: TrainingCallbackAttributes) -> List[TrainingCallback]:

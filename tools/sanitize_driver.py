@@ -3,7 +3,8 @@ fixed + occupancy march, visibility mask, fused field forward (inference and tra
 several tiles per CTA so the mbarrier ring / tile counters wrap), composite fwd/bwd, losses, field / deformation
 backward, rank-1 expand + fused Adam, occupancy update, component kernels, surface normals (canonical and observation
 space), the deformation input gradient (ragged last tile, a device sample count below the buffer size), the mesh export
-(a ragged last tile of grid points, an occupancy grid, vertex normals and colours)."""
+(a ragged last tile of grid points, an occupancy grid, vertex normals and colours), the deformation Jacobian and inverse
+(ragged last tile, several tiles per CTA, per-sample warp codes) and a tracked mesh sequence."""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
@@ -40,6 +41,14 @@ ops.field_forward(P, window_hash=32.0, window_deform=7.0, positions=P.aabb[0].to
                   sample_times=torch.rand(500, device=dev), want=("sigma",))
 ops.extract_mesh(P, time=0.5, level=0.5, resolution=(13, 11, 9), window_hash=32.0, window_deform=7.0,
                  binaries=torch.rand((1, 16, 16, 16), device=dev) > 0.3, aabbs=P.aabb.reshape(1, 6).to(dev))
+xw = P.aabb[0].to(dev) + torch.rand((4100, 3), device=dev) * (P.aabb[1] - P.aabb[0]).to(dev)
+tw = torch.rand(4100, device=dev)
+ops.deform_jacobian(P, window_deform=3.3, positions=xw, sample_times=tw)
+ops.deform_jacobian(P, positions=xw[:500], sample_warp_codes=torch.randn((500, 128), device=dev) * 0.1)
+ops.deform_inverse(P, xw, sample_times=tw, window_deform=3.3, max_iter=5)
+ops.track_points(P, xw[:77], time_from=0.25, times_to=[0.0, 1.0], window_deform=7.0)
+ops.extract_mesh_sequence(P, times=[0.0, 1.0], reference_time=0.5, level=0.5, resolution=(13, 11, 9), window_hash=32.0,
+                          window_deform=7.0)
 # plugin model: occupancy march + pre-pass + training step + occupancy update
 m = bench.build_model(S, dev).train()
 occ = bench.blob_occupancy(seed=5)
