@@ -31,6 +31,9 @@
  *                          positions (an extension: the reference never differentiates the warp by position)
  *   nsb_deform_jacobian / nsb_deform_inverse
  *                          the warp's Jacobian and its inverse (an extension: point tracking across timesteps)
+ *   nsb_flow_select / nsb_flow_composite
+ *                          scene flow and optical flow of a render between timesteps (an extension: the reference
+ *                          renders only the canonical offset, nersemble_deformation_renderer.py)
  *   nsb_table_adam_step    torch.optim.Adam on the 8 tcnn grid tensors (scripts/train/train_nersemble.py:243-247) and
  *                          tcnn's per-call fp32 -> fp16 cast of the table parameters
  */
@@ -547,6 +550,58 @@ typedef struct {
 } nsb_mesh_args;
 int nsb_mesh_count(const nsb_mesh_args *args, void *stream);
 int nsb_mesh_emit(const nsb_mesh_args *args, void *stream);
+
+/* Scene flow and optical flow of a render between timesteps (an extension; DESIGN 4.2f), from the packed samples, weights
+ * and offsets nsb_render_forward left in its workspace, without a host synchronisation:
+ *   select     -> nsb_deform_inverse (positions = targets, init, sample_times = the target time,
+ *                 n_samples = capacity, n_samples_dev = n_selected) -> composite.
+ * nsb_flow_select: packed sample i of ray r (i in r's packed_info segment and i < *n_total) is selected iff
+ * weights[i] >= min_weight.  Its world midpoint x = o + d (ts + te) / 2 (formed like the field kernels) and its canonical
+ * target c = x + offsets[i] are written in (ray, sample) order; ray_sel[r] = (start, count) of r's selection and
+ * *n_selected the total.  The ray of a sample is the owner of its segment, so ray_indices are not read.  Passes: per-ray
+ * counts | exclusive scan of the per-tile sums | fill, no atomics (the same bits on every run).  The outputs hold
+ * `capacity` entries because only the device knows the count.
+ * nsb_flow_composite: per ray, over its selected samples j whose inverse converged (status NSB_INV_CONVERGED), with
+ * w = weights[sel_index[j]], x = init[j], x' = positions[j], summed in selection order in fp32:
+ *   flow_weight = W = sum w,  scene_flow = sum w (x' - x) / W (0 when W = 0),
+ *   optical_flow = sum w (pi(x') - pi(x)) / sum w over the samples whose two positions are in front of the camera (0
+ *   when there is none), in pixels (dx right, dy down); pi inverts nsb_ray_batch's pinhole model:
+ *   Xc = R^T (X - o), pi(X) = (cx + fx Xc.x / -Xc.z, cy - fy Xc.y / -Xc.z).  The principal point cancels in the
+ *   difference.  optical_flow NULL: no camera, intrinsics / camera_to_world are not read. */
+#define NSB_FLOW_TILE 64        /* rays per CTA of the selection passes (8 per warp) */
+typedef struct {
+    int64_t n_rays;
+    int64_t capacity;             /* > 0: entries of the render's per-sample arrays and of the selection outputs */
+    const int64_t *packed_info;   /* [n_rays][2] (start, count) of the render */
+    const float *t_starts, *t_ends, *weights; /* [capacity] */
+    const float *offsets;         /* [capacity][3] */
+    const float *origins, *directions; /* [n_rays][3] */
+    const int64_t *n_total;       /* device scalar: packed samples of the render (nsb_render_ws_header.n_total) */
+    float min_weight;             /* finite, in [0, 1) */
+    int64_t *ray_sel;             /* [n_rays][2] out: (start, count) of each ray's selection */
+    int64_t *sel_index;           /* [capacity] out: packed sample index */
+    float *targets;               /* [capacity][3] out: c = x + offset (world) */
+    float *init;                  /* [capacity][3] out: x (world) */
+    int64_t *n_selected;          /* device scalar out */
+    int64_t *tile_sums;           /* [ceil(n_rays / NSB_FLOW_TILE)] workspace */
+} nsb_flow_select_args;
+int nsb_flow_select(const nsb_flow_select_args *args, void *stream);
+typedef struct {
+    int64_t n_rays;
+    int64_t capacity;             /* > 0, as in nsb_flow_select_args */
+    const int64_t *ray_sel;       /* [n_rays][2], nsb_flow_select's */
+    const int64_t *sel_index;     /* [capacity] */
+    const float *init;            /* [capacity][3] */
+    const float *positions;       /* [capacity][3]: nsb_deform_inverse's positions */
+    const int32_t *status;        /* [capacity]: nsb_deform_inverse's status */
+    const float *weights;         /* [capacity] render weights */
+    float intrinsics[4];          /* fx, fy (> 0), cx, cy; finite */
+    float camera_to_world[12];    /* [3][4] row-major; finite */
+    float *scene_flow;            /* [n_rays][3] out, world units */
+    float *flow_weight;           /* [n_rays] out */
+    float *optical_flow;          /* [n_rays][2] out or NULL (no camera) */
+} nsb_flow_composite_args;
+int nsb_flow_composite(const nsb_flow_composite_args *args, void *stream);
 
 /* Training sampler WITHOUT host synchronisation (model_components/nersemble_volumetric_sampler.py:95-108 around nerfacc
  * OccGridEstimator.sampling): (1) nsb_march_occupancy_packed = count/scan/fill of nsb_march_occupancy as ONE cooperative

@@ -175,6 +175,24 @@ class MeshArgs(C.Structure):       # nsb_mesh_args
 MESH_TILE = 1024        # NSB_MESH_TILE
 
 
+class FlowSelectArgs(C.Structure):  # nsb_flow_select_args
+    _fields_ = [("n_rays", C.c_int64), ("capacity", C.c_int64), ("packed_info", C.c_void_p), ("t_starts", C.c_void_p),
+                ("t_ends", C.c_void_p), ("weights", C.c_void_p), ("offsets", C.c_void_p), ("origins", C.c_void_p),
+                ("directions", C.c_void_p), ("n_total", C.c_void_p), ("min_weight", C.c_float), ("ray_sel", C.c_void_p),
+                ("sel_index", C.c_void_p), ("targets", C.c_void_p), ("init", C.c_void_p), ("n_selected", C.c_void_p),
+                ("tile_sums", C.c_void_p)]
+
+
+class FlowCompositeArgs(C.Structure):  # nsb_flow_composite_args
+    _fields_ = [("n_rays", C.c_int64), ("capacity", C.c_int64), ("ray_sel", C.c_void_p), ("sel_index", C.c_void_p),
+                ("init", C.c_void_p), ("positions", C.c_void_p), ("status", C.c_void_p), ("weights", C.c_void_p),
+                ("intrinsics", C.c_float * 4), ("camera_to_world", C.c_float * 12), ("scene_flow", C.c_void_p),
+                ("flow_weight", C.c_void_p), ("optical_flow", C.c_void_p)]
+
+
+FLOW_TILE = 64          # NSB_FLOW_TILE
+
+
 class RenderWsHeader(C.Structure):
     _fields_ = [("barrier", C.c_uint32), ("depth_range", C.c_uint32 * 2), ("status", C.c_int32), ("n_total", C.c_int64),
                 ("reserved", C.c_int64 * 5)]
@@ -230,6 +248,8 @@ SYMBOLS = {
                                       C.POINTER(NormalsArgs), C.c_void_p]),
     "nsb_mesh_count": (C.c_int, [C.POINTER(MeshArgs), C.c_void_p]),
     "nsb_mesh_emit": (C.c_int, [C.POINTER(MeshArgs), C.c_void_p]),
+    "nsb_flow_select": (C.c_int, [C.POINTER(FlowSelectArgs), C.c_void_p]),
+    "nsb_flow_composite": (C.c_int, [C.POINTER(FlowCompositeArgs), C.c_void_p]),
 }
 
 _lib = None

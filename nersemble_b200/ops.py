@@ -370,6 +370,10 @@ def deform_input_grad(P: NativeParams, u: torch.Tensor, *, window_deform=None, l
 # orders of magnitude below fp16's maximum (65504) while the entries that matter stay far above its smallest normal (6.1e-5).
 JVP_TANGENT_SCALE = 1.0 / 16.0
 INVERSE_MAX_ITER = 64
+# Render weight below which a sample takes no part in render_flow (DESIGN 4.2f): such samples are nearly transparent space,
+# and inverting the warp for them is most of the cost of a flow pass for almost none of its weight.
+# accumulation - flow_weight reports, per ray, the weight this leaves out.
+FLOW_MIN_WEIGHT = 1e-3
 
 
 def _positions_samples(sample_kw, who: str):
@@ -418,7 +422,8 @@ def _check_newton(max_iter, tol, who: str):
 
 def deform_inverse(P: NativeParams, targets: torch.Tensor, *, sample_times: Optional[torch.Tensor] = None,
                    uniform_time: Optional[float] = None, init: Optional[torch.Tensor] = None, window_deform=None,
-                   sample_warp_codes: Optional[torch.Tensor] = None, max_iter: int = 20, tol: float = 1e-4) -> Dict[str, torch.Tensor]:
+                   sample_warp_codes: Optional[torch.Tensor] = None, max_iter: int = 20, tol: float = 1e-4,
+                   n_samples_dev: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
     """Inverse of the deformation (nsb_deform_inverse): for each target c [n,3] -- a world position of the warped hash
     input, i.e. an observed position plus its normalised offset, as the field kernels form it -- the observed position p
     whose warp at the given time lands on c: the root of p_n + D^-1 offset(p_n) - c_n by damped Newton in the kernel.
@@ -426,7 +431,8 @@ def deform_inverse(P: NativeParams, targets: torch.Tensor, *, sample_times: Opti
     init [n,3]: initial guesses (default: the targets).  tol: on |F|inf in normalised units (1e-4 is about 1/20 of a voxel
     of a 512^3 grid).  Returns {"positions" [n,3] world (the best trial; the initial guess bit for bit when it already
     converged), "residual" [n] (|F|inf there), "iterations" [n] int32, "converged" [n] bool, "status" [n] int32
-    (_lib.INV_CONVERGED / INV_NOT_CONVERGED / INV_SINGULAR)}.  Not differentiable."""
+    (_lib.INV_CONVERGED / INV_NOT_CONVERGED / INV_SINGULAR)}.  n_samples_dev: optional device int64 scalar, the number of
+    leading points to solve (the rest of every output is left as it was allocated).  Not differentiable."""
     _check_newton(max_iter, tol, "deform_inverse")
     if (sample_times is not None) + (uniform_time is not None) + (sample_warp_codes is not None) > 1:
         raise ValueError("deform_inverse: give one of sample_times, uniform_time, sample_warp_codes")
@@ -440,6 +446,9 @@ def deform_inverse(P: NativeParams, targets: torch.Tensor, *, sample_times: Opti
     _fill_samples(s, keep, positions=targets, sample_times=sample_times)
     if sample_warp_codes is not None:
         _fill_sample_code_bias(P, s, keep, sample_warp_codes, n, dev)
+    if n_samples_dev is not None:
+        assert n_samples_dev.dtype == torch.int64 and n_samples_dev.is_cuda and n_samples_dev.numel() == 1
+        s.n_samples_dev = _ptr(n_samples_dev); keep.append(n_samples_dev)
     a = _lib.DeformInvArgs()
     if init is not None:
         init = _f32c(init).reshape(-1, 3)
@@ -1207,6 +1216,86 @@ def render_rays(P: NativeParams, origins, directions, ray_times, *, window_hash=
                               observation=use_deformation and normals_space == "observation")
         buf["normals"] = nrm["normals"]
         out["normals"] = nrm["ray_normals"]
+    return out
+
+
+def _flow_camera(camera, who: str):
+    """(intrinsics (fx, fy, cx, cy), camera_to_world [3,4]) as host floats; a CUDA tensor is copied (one synchronisation)."""
+    import math
+    if not (isinstance(camera, (tuple, list)) and len(camera) == 2):
+        raise ValueError(f"{who}: camera must be (intrinsics [4], camera_to_world [3,4])")
+    intr = [float(v) for v in torch.as_tensor(camera[0]).detach().reshape(-1).tolist()]
+    c2w = [float(v) for v in torch.as_tensor(camera[1]).detach().reshape(-1).tolist()]
+    if len(intr) != 4 or len(c2w) != 12:
+        raise ValueError(f"{who}: camera must be (intrinsics [4], camera_to_world [3,4])")
+    if not all(math.isfinite(v) for v in intr + c2w):
+        raise ValueError(f"{who}: camera values must be finite")
+    if not (intr[0] > 0 and intr[1] > 0):
+        raise ValueError(f"{who}: fx and fy must be > 0")
+    return intr, c2w
+
+
+def render_flow(P: NativeParams, result: RenderResult, origins, directions, ray_times, *, time_to: float,
+                window_deform=None, camera=None, min_weight: float = FLOW_MIN_WEIGHT, max_iter: int = 20,
+                tol: float = 1e-4) -> Dict[str, torch.Tensor]:
+    """Scene flow and optical flow of a render_rays result from the rays' own times to `time_to` (DESIGN 4.2f), without a
+    host synchronisation: nsb_flow_select picks the render's packed samples with weight >= min_weight, nsb_deform_inverse
+    moves each one's canonical target c = x + offset to time_to (init x, the selected count on the device) and
+    nsb_flow_composite averages the motion per ray.  origins / directions / ray_times: the ones the render was given;
+    window_deform: the render's.  camera: optional (intrinsics (fx, fy, cx, cy), camera_to_world [3,4]) in the
+    DeviceImageCache form, as host values (a CUDA tensor costs one synchronisation).
+    Returns {"scene_flow" [R,3] world units, "flow_weight" [R,1] (the render weight the flow represents; accumulation -
+    flow_weight was left out), "optical_flow" [R,2] pixels (dx right, dy down; with a camera)} plus, for tests, the
+    selection ("_ray_sel" [R,2], "_sel_index", "_targets", "_init", "_n_selected") and the inverse ("_inverse"), all
+    sized by the render's capacity.  Without deformation every time is the same space: zero flow, flow_weight =
+    accumulation, and no flow kernel runs.  The flow follows the deformation only; occlusion at time_to is not handled."""
+    import math
+    _check_newton(max_iter, tol, "render_flow")
+    if not (math.isfinite(float(time_to)) and 0.0 <= float(time_to) <= 1.0):
+        raise ValueError(f"render_flow: time_to must be in [0, 1], got {time_to!r}")
+    if not (math.isfinite(float(min_weight)) and 0.0 <= float(min_weight) < 1.0):
+        raise ValueError(f"render_flow: min_weight must be finite and in [0, 1), got {min_weight!r}")
+    cam = None if camera is None else _flow_camera(camera, "render_flow")
+    acc = result["accumulation"]
+    dev, R = acc.device, int(acc.shape[0])
+    buf = result["_buffers"]
+    out = {"scene_flow": torch.zeros((R, 3), dtype=_F32, device=dev)}
+    if cam is not None:
+        out["optical_flow"] = torch.zeros((R, 2), dtype=_F32, device=dev)
+    if buf["offsets"] is None:
+        out["flow_weight"] = acc.clone()
+        return out
+    out["flow_weight"] = torch.empty((R, 1), dtype=_F32, device=dev)
+    lib = _lib.load()
+    origins, directions = _f32c(origins).reshape(-1, 3), _f32c(directions).reshape(-1, 3)
+    _need_cuda(origins, directions)
+    assert origins.shape[0] == R and directions.shape[0] == R, (origins.shape, directions.shape, R)
+    cap = int(buf["capacity"])
+    sel = {"_ray_sel": torch.empty((R, 2), dtype=torch.int64, device=dev),
+           "_sel_index": torch.empty((cap,), dtype=torch.int64, device=dev),
+           "_targets": torch.empty((cap, 3), dtype=_F32, device=dev), "_init": torch.empty((cap, 3), dtype=_F32, device=dev),
+           "_n_selected": torch.empty((1,), dtype=torch.int64, device=dev)}
+    tiles = torch.empty((max((R + _lib.FLOW_TILE - 1) // _lib.FLOW_TILE, 1),), dtype=torch.int64, device=dev)
+    a = _lib.FlowSelectArgs()
+    a.n_rays, a.capacity, a.packed_info = R, cap, _ptr(result["packed_info"])
+    a.t_starts, a.t_ends, a.weights, a.offsets = _ptr(buf["t_starts"]), _ptr(buf["t_ends"]), _ptr(buf["weights"]), _ptr(buf["offsets"])
+    a.origins, a.directions, a.n_total, a.min_weight = _ptr(origins), _ptr(directions), _ptr(buf["header"][2:3]), float(min_weight)
+    a.ray_sel, a.sel_index, a.targets, a.init = _ptr(sel["_ray_sel"]), _ptr(sel["_sel_index"]), _ptr(sel["_targets"]), _ptr(sel["_init"])
+    a.n_selected, a.tile_sums = _ptr(sel["_n_selected"]), _ptr(tiles)
+    _lib.check(lib.nsb_flow_select(C.byref(a), _stream()), "nsb_flow_select")
+    inv = deform_inverse(P, sel["_targets"], uniform_time=float(time_to), init=sel["_init"], window_deform=window_deform,
+                         max_iter=max_iter, tol=tol, n_samples_dev=sel["_n_selected"])
+    c = _lib.FlowCompositeArgs()
+    c.n_rays, c.capacity, c.ray_sel, c.sel_index = R, cap, _ptr(sel["_ray_sel"]), _ptr(sel["_sel_index"])
+    c.init, c.positions, c.status, c.weights = _ptr(sel["_init"]), _ptr(inv["positions"]), _ptr(inv["status"]), _ptr(buf["weights"])
+    c.scene_flow, c.flow_weight = _ptr(out["scene_flow"]), _ptr(out["flow_weight"])
+    if cam is not None:
+        c.intrinsics[:] = cam[0]
+        c.camera_to_world[:] = cam[1]
+        c.optical_flow = _ptr(out["optical_flow"])
+    _lib.check(lib.nsb_flow_composite(C.byref(c), _stream()), "nsb_flow_composite")
+    out.update(sel)
+    out["_inverse"] = inv
     return out
 
 

@@ -338,6 +338,40 @@ class NeRSembleNGPModel(Model):
         return {k: out[k] for k in ("positions", "residual", "converged")}
 
     @torch.no_grad()
+    def render_flow(self, camera_ray_bundle: RayBundle, timestep_to: int, intrinsics=None, camera_to_world=None,
+                    max_iter: int = 20, tol: float = 1e-4) -> Dict[str, Tensor]:
+        """get_outputs_for_camera_ray_bundle's outputs of an [H, W] bundle (same chunks, windows and per-frame table) plus
+        the motion of each pixel's surface to frame `timestep_to` (ops.render_flow, DESIGN 4.2f): "scene_flow" [H,W,3]
+        (world units), "flow_weight" [H,W,1] (the part of accumulation the flow represents) and, with a camera in the
+        DeviceImageCache form (intrinsics (fx, fy, cx, cy), camera_to_world [3,4]), "optical_flow" [H,W,2] in pixels
+        (dx right, dy down).  The flow follows the deformation only and ignores occlusion in frame timestep_to.  Without a
+        deformation field the flow is 0 and flow_weight equals accumulation."""
+        t_to = self._timestep_time(timestep_to)
+        if (intrinsics is None) != (camera_to_world is None):
+            raise ValueError("render_flow: give both intrinsics and camera_to_world, or neither")
+        if not self.scene_aabb.is_cuda:
+            raise RuntimeError("render_flow needs the model on CUDA (there is no CPU fallback)")
+        camera = None if intrinsics is None else ops._flow_camera((intrinsics, camera_to_world), "render_flow")
+        n = self.config.eval_num_rays_per_chunk
+        h, w = camera_ray_bundle.origins.shape[:2]
+        uniform_time = self._frame_uniform_time(camera_ray_bundle)
+        _, wd = self._windows()
+        lists: Dict[str, list] = {}
+        for i in range(0, h * w, n):
+            rb = camera_ray_bundle.get_row_major_sliced_ray_bundle(i, i + n)
+            res = self._fused_render(rb, uniform_time)
+            flow = ops.render_flow(self.native_params(), res, rb.origins.reshape(-1, 3), rb.directions.reshape(-1, 3),
+                                   self._ray_times(rb), time_to=t_to, window_deform=wd, camera=camera, max_iter=max_iter,
+                                   tol=tol)
+            for name in ("rgb", "accumulation", "depth", "num_samples_per_ray", "deformation", "normals"):
+                if name in res:
+                    lists.setdefault(name, []).append(res[name])
+            for name in ("scene_flow", "flow_weight", "optical_flow"):
+                if name in flow:
+                    lists.setdefault(name, []).append(flow[name])
+        return {k: torch.cat(v).view(h, w, -1) for k, v in lists.items()}
+
+    @torch.no_grad()
     def extract_mesh_sequence(self, timesteps, reference_timestep: int, resolution=256, level: Optional[float] = None,
                               space: str = "observation", respect_occupancy: bool = True, box=None, normals: bool = True,
                               colours: bool = True) -> MeshSequence:
@@ -473,6 +507,18 @@ class NeRSembleNGPModel(Model):
     def _fused_ok(self) -> bool:
         return self.use_fused_render and not self.sampler.training and self.scene_aabb.is_cuda
 
+    def _frame_uniform_time(self, camera_ray_bundle: RayBundle) -> Optional[float]:
+        """A camera frame has ONE timestep (evaluate_nersemble.py renders camera x timestep): when all rays carry the same
+        time (checked here: one host synchronisation per FRAME), the 32-member blend is hoisted out of the per-sample
+        path into a per-frame table (ops.NativeParams.frame_table) that every chunk of the frame gathers from L2."""
+        h, w = camera_ray_bundle.origins.shape[:2]
+        if (self.frame_tables and camera_ray_bundle.times is not None and self.config.use_hash_ensemble
+                and h * w >= self.frame_table_min_rays):
+            t = camera_ray_bundle.times
+            lo, hi = torch.stack([t.min(), t.max()]).tolist()
+            return lo if lo == hi else None
+        return None
+
     @torch.no_grad()
     def get_outputs_for_camera_ray_bundle(self, camera_ray_bundle: RayBundle) -> Dict[str, Tensor]:
         """nerfstudio Model.get_outputs_for_camera_ray_bundle (the eval entry point: evaluate_nersemble.py:143,
@@ -482,15 +528,7 @@ class NeRSembleNGPModel(Model):
             return super().get_outputs_for_camera_ray_bundle(camera_ray_bundle)
         n = self.config.eval_num_rays_per_chunk
         h, w = camera_ray_bundle.origins.shape[:2]
-        # A camera frame has ONE timestep (evaluate_nersemble.py renders camera x timestep): when all rays carry the same
-        # time (checked here: one host synchronisation per FRAME), the 32-member blend is hoisted out of the per-sample
-        # path into a per-frame table (ops.NativeParams.frame_table) that every chunk of the frame gathers from L2.
-        uniform_time = None
-        if (self.frame_tables and camera_ray_bundle.times is not None and self.config.use_hash_ensemble
-                and h * w >= self.frame_table_min_rays):
-            t = camera_ray_bundle.times
-            lo, hi = torch.stack([t.min(), t.max()]).tolist()
-            uniform_time = lo if lo == hi else None
+        uniform_time = self._frame_uniform_time(camera_ray_bundle)
         lists: Dict[str, list] = {}
         for i in range(0, h * w, n):
             rb = camera_ray_bundle.get_row_major_sliced_ray_bundle(i, i + n)

@@ -4,7 +4,8 @@ several tiles per CTA so the mbarrier ring / tile counters wrap), composite fwd/
 backward, rank-1 expand + fused Adam, occupancy update, component kernels, surface normals (canonical and observation
 space), the deformation input gradient (ragged last tile, a device sample count below the buffer size), the mesh export
 (a ragged last tile of grid points, an occupancy grid, vertex normals and colours), the deformation Jacobian and inverse
-(ragged last tile, several tiles per CTA, per-sample warp codes) and a tracked mesh sequence."""
+(ragged last tile, several tiles per CTA, per-sample warp codes), a tracked mesh sequence, and the flow pass (selection
+of a fixed-stride render, the inverse over the device-side selected count, compositing with a camera)."""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
@@ -49,6 +50,11 @@ ops.deform_inverse(P, xw, sample_times=tw, window_deform=3.3, max_iter=5)
 ops.track_points(P, xw[:77], time_from=0.25, times_to=[0.0, 1.0], window_deform=7.0)
 ops.extract_mesh_sequence(P, times=[0.0, 1.0], reference_time=0.5, level=0.5, resolution=(13, 11, 9), window_hash=32.0,
                           window_deform=7.0)
+cam = ((300.0, 310.0, 32.0, 24.0), torch.tensor([[1.0, 0.0, 0.0, 0.1], [0.0, 1.0, 0.0, 0.2], [0.0, 0.0, 1.0, 9.0]]))
+rf = ops.render_rays(P, o, d, t, window_hash=32.0, window_deform=7.0, sampler="fixed", n_per_ray=100, near_plane=bench.NEAR,
+                     step=bench.STEP)
+ops.render_flow(P, rf, o, d, t, time_to=0.75, window_deform=7.0, camera=cam, max_iter=5)
+ops.render_flow(P, rf, o, d, t, time_to=0.0, window_deform=7.0)
 # plugin model: occupancy march + pre-pass + training step + occupancy update
 m = bench.build_model(S, dev).train()
 occ = bench.blob_occupancy(seed=5)
