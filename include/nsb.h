@@ -34,6 +34,9 @@
  *   nsb_flow_select / nsb_flow_composite
  *                          scene flow and optical flow of a render between timesteps (an extension: the reference
  *                          renders only the canonical offset, nersemble_deformation_renderer.py)
+ *   nsb_render_forward_interp
+ *                          nsb_render_forward between captured timesteps (an extension: the reference rounds a ray's
+ *                          time to the nearest timestep, nersemble_instant_ngp.py:301-303)
  *   nsb_table_adam_step    torch.optim.Adam on the 8 tcnn grid tensors (scripts/train/train_nersemble.py:243-247) and
  *                          tcnn's per-call fp32 -> fp16 cast of the table parameters
  */
@@ -484,6 +487,15 @@ typedef struct nsb_render_ws_header {  /* first 64 bytes of the workspace; n_tot
 } nsb_render_ws_header;
 size_t nsb_render_workspace_bytes(int64_t n_rays);
 int nsb_render_forward(const nsb_field_params *params, const nsb_field_opts *opts, const nsb_render_args *args, void *stream);
+/* nsb_render_forward at continuous ray times (an extension; DESIGN 4.2g).  A ray of time t samples the field at the
+ * fractional timestep u = clamp(t (T - 1), 0, T - 1), snapped to round(u) within 2^-10 timesteps; with i0 = floor(u),
+ * i1 = min(i0 + 1, T - 1) and lam = u - i0, every per-timestep quantity is fmaf(lam, q[i1] - q[i0], q[i0]): the
+ * entries of the timestep stack (frame_table with frame_stride >= the total entry count) before the trilinear weights,
+ * or else the blend_codes rows before the member fold, and the deform_code_bias rows of layers 0 and 4.  At an integer u
+ * the outputs are those of nsb_render_forward bit for bit.  Needs use_deformation and deform_packed_umma; a frame
+ * table that is not such a stack is rejected.  Same arguments, outputs and absence of host synchronisation otherwise. */
+int nsb_render_forward_interp(const nsb_field_params *params, const nsb_field_opts *opts, const nsb_render_args *args,
+                              void *stream);
 
 /* Surface normals of the density field (nerfstudio Field.get_normals, used by NeRSembleNeRFactoField.forward with
  * compute_normals=True: nerfstudio/fields/nersemble_nerfacto_field.py:385-402) and their per-ray composite

@@ -244,6 +244,7 @@ SYMBOLS = {
     "nsb_visibility_compact": (C.c_int, [C.POINTER(VisCompactArgs), C.c_void_p]),
     "nsb_vis_compact_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64]),
     "nsb_render_forward": (C.c_int, [C.POINTER(FieldParams), C.POINTER(FieldOpts), C.POINTER(RenderArgs), C.c_void_p]),
+    "nsb_render_forward_interp": (C.c_int, [C.POINTER(FieldParams), C.POINTER(FieldOpts), C.POINTER(RenderArgs), C.c_void_p]),
     "nsb_normals_forward": (C.c_int, [C.POINTER(FieldParams), C.POINTER(FieldOpts), C.POINTER(Samples),
                                       C.POINTER(NormalsArgs), C.c_void_p]),
     "nsb_mesh_count": (C.c_int, [C.POINTER(MeshArgs), C.c_void_p]),

@@ -52,6 +52,20 @@ __device__ __forceinline__ int sample_timestep(float t, int n_timesteps) {
     return min(max(ts, 0), n_timesteps - 1);
 }
 
+// Continuous time (DESIGN 4.2g, the linear render kernels): the fractional timestep u = clamp(t * (T - 1), 0, T - 1),
+// snapped to the nearest integer within NSB_TIME_SNAP timesteps (fp32 times k / (T - 1) land a few ulp off k).  A
+// snapped u equals sample_timestep(t).  The rows interpolated are floor(u) and min(floor(u) + 1, T - 1) at
+// lam = u - floor(u) (exact in fp32); ops.time_lerp is the host mirror.
+#define NSB_TIME_SNAP 0.0009765625f     // 2^-10 timesteps
+__device__ __forceinline__ float sample_time_u(float t, int n_timesteps) {
+    const float tm = (float)(n_timesteps - 1);
+    const float u = fminf(fmaxf(__fmul_rn(t, tm), 0.f), tm);
+    const float r = rintf(u);
+    return fabsf(u - r) <= NSB_TIME_SNAP ? r : u;
+}
+// (1 - lam) a + lam b, exactly a at lam = 0
+__device__ __forceinline__ float time_lerp(float a, float b, float lam) { return fmaf(lam, b - a, a); }
+
 // One axis of a ray sample's position: o + d * (t_start + t_end) / 2, with mid = t_start + t_end (no FMA, like the oracle).
 __device__ __forceinline__ float ray_midpoint(float o, float d, float mid) {
     return __fadd_rn(o, __fmul_rn(__fmul_rn(d, mid), 0.5f));

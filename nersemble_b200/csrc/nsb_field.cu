@@ -300,7 +300,7 @@ __global__ void __launch_bounds__(kLaunchBoundWS, 1) field_kernel_ws(const __gri
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     SmemWS &sm = *reinterpret_cast<SmemWS *>(smem_raw);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    constexpr bool FEAT_GIVEN = false;
+    constexpr bool FEAT_GIVEN = false, LERP = false;
     // NOTE: nothing is computed ahead of the role split on purpose.  Values shared by both roles get registers that
     // suit the 88-register tensor role, and the 64-register gather role then pays for them with spills inside its
     // sample loop.  Each role derives its loop bounds itself.
@@ -328,7 +328,7 @@ __global__ void __launch_bounds__(kLaunchBoundWS, 1) field_kernel_ws_given(const
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     SmemWS &sm = *reinterpret_cast<SmemWS *>(smem_raw);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    constexpr bool FIELD = true, HEAD = true, SAVE = true, FEAT_GIVEN = true;
+    constexpr bool FIELD = true, HEAD = true, SAVE = true, FEAT_GIVEN = true, LERP = false;
 #define NSB_N_SAMPLES A.S.n_samples
 #include "nsb_field_setup.inc"
     if (warp >= kTensorWarps) {
@@ -449,7 +449,7 @@ __global__ void __launch_bounds__(kLaunchBoundWS, 1) field_kernel_tc(const __gri
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     SmemTC &sm = *reinterpret_cast<SmemTC *>(smem_raw);
     const int tid = threadIdx.x, lane = tid & 31, warp = tc_warp_index(tid);
-    constexpr bool FIELD = true, SAVE = false, FEAT_GIVEN = false;
+    constexpr bool FIELD = true, SAVE = false, FEAT_GIVEN = false, LERP = false;
 #define NSB_N_SAMPLES A.S.n_samples
     NSB_TC_SETUP()
     if (warp >= kTensorWarps) {
@@ -474,7 +474,7 @@ __global__ void __launch_bounds__(kLaunchBoundWS, 1) field_kernel_ws_dyn(const _
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     SmemWS &sm = *reinterpret_cast<SmemWS *>(smem_raw);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    constexpr bool FEAT_GIVEN = false;
+    constexpr bool FEAT_GIVEN = false, LERP = false;
     if (tid == 0) sm.n_dyn = min(*A.S.n_samples_dev, A.S.n_samples);      // visible after the setup's __syncthreads
 #define NSB_N_SAMPLES (*reinterpret_cast<const volatile int64_t *>(&sm.n_dyn))
 #include "nsb_field_setup.inc"
@@ -620,7 +620,7 @@ __global__ void __launch_bounds__(kLaunchBoundWS, 1) render_kernel_ws(const __gr
     SmemWS &sm = *reinterpret_cast<SmemWS *>(smem_raw);
     const FieldArgs &A = K.F;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    constexpr bool FIELD = true, HEAD = true, SAVE = false, FEAT_GIVEN = false;
+    constexpr bool FIELD = true, HEAD = true, SAVE = false, FEAT_GIVEN = false, LERP = false;
 
 #define NSB_N_SAMPLES (*reinterpret_cast<const volatile int64_t *>(&sm.n_dyn))
     if (tid == 0) mbar_init(&sm.sampler_done, 1);                          // fenced + published by the setup below
@@ -650,7 +650,7 @@ __global__ void __launch_bounds__(kLaunchBoundWS, 1) render_kernel_tc(const __gr
     SmemTC &sm = *reinterpret_cast<SmemTC *>(smem_raw);
     const FieldArgs &A = K.F;
     const int tid = threadIdx.x, lane = tid & 31, warp = tc_warp_index(tid);
-    constexpr bool FIELD = true, HEAD = true, SAVE = false, FEAT_GIVEN = false;
+    constexpr bool FIELD = true, HEAD = true, SAVE = false, FEAT_GIVEN = false, LERP = false;
 #define NSB_N_SAMPLES (*reinterpret_cast<const volatile int64_t *>(&sm.n_dyn))
     KPROF(0)
     if (tid == 0) mbar_init(&sm.sampler_done, 1);
@@ -677,6 +677,42 @@ __global__ void __launch_bounds__(kLaunchBoundWS, 1) render_kernel_tc(const __gr
     KPROF(3)
     render_composite_phase(K);
     KPROF(4)
+}
+
+// render_kernel_tc at continuous ray times (nsb_render_forward_interp, DESIGN 4.2g): the same role bodies with LERP set.
+// Every row carries its fractional timestep u (sample_time_u) in xs.w and row_ts instead of its timestep; the gather
+// interpolates the stack entries (FRAME = STACK = true) or the blend codes (FRAME = STACK = false) of floor(u) and
+// floor(u) + 1, the tensor role the code-bias rows of layers 0 and 4.  Its own name: a fourth template flag on
+// render_kernel_tc would give the existing kernels new symbols.
+template <int SAMPLER, bool FRAME, bool STACK>
+__global__ void __launch_bounds__(kLaunchBoundWS, 1) render_kernel_tc_lerp(const __grid_constant__ RenderKArgs K) {
+    extern __shared__ __align__(1024) uint8_t smem_raw[];
+    SmemTC &sm = *reinterpret_cast<SmemTC *>(smem_raw);
+    const FieldArgs &A = K.F;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tc_warp_index(tid);
+    constexpr bool FIELD = true, HEAD = true, SAVE = false, FEAT_GIVEN = false, LERP = true;
+    static_assert(FRAME == STACK, "linear time: the timestep stack or the per-sample blend");
+#define NSB_N_SAMPLES (*reinterpret_cast<const volatile int64_t *>(&sm.n_dyn))
+    if (tid == 0) mbar_init(&sm.sampler_done, 1);
+    NSB_TC_SETUP()
+    if (warp >= kTensorWarps) {
+        if (kGatherRegs != kLaunchRegs) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kGatherRegs));
+        mbar_wait<200>(&sm.sampler_done, 0);
+        if constexpr (FRAME) {
+#include "nsb_field_gather_role_frame.inc"
+        } else {
+#include "nsb_field_gather_role.inc"
+        }
+        return;
+    }
+    if (kTensorRegs != kLaunchRegs) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kTensorRegs));
+    render_sampler_phase<SAMPLER, SmemTC>(K);
+    if (tid == 0) mbar_arrive(&sm.sampler_done);
+    {
+#include "nsb_field_tensor_role_tc.inc"
+    }
+#undef NSB_N_SAMPLES
+    render_composite_phase(K);
 }
 
 // -------------------------------------------------------------------------------------------
@@ -956,28 +992,53 @@ extern "C" size_t nsb_render_workspace_bytes(int64_t n_rays) {
     return kRenderHdrBytes + kRenderPartials * sizeof(int64_t) + (size_t)std::max<int64_t>(n_rays, 1) * sizeof(int32_t) + 64;
 }
 
-extern "C" int nsb_render_forward(const nsb_field_params *params, const nsb_field_opts *opts, const nsb_render_args *ra, void *stream) {
-    if (!params || !opts || !ra) { set_error("nsb_render_forward: null argument"); return 1; }
+namespace nsb {
+template <int SAMPLER, bool FR>
+static int launch_render_tc_lerp_(const RenderKArgs &K, cudaStream_t st) {
+    if (!tc_args_ok(K.F)) return 1;
+    return launch_persistent<render_kernel_tc_lerp<SAMPLER, FR, FR>>(K, tc_smem_bytes<FR>(tc_code_bias_rows<FR>(K.F.P.n_timesteps)),
+                                                                     tc_smem_bytes<FR>(tc_code_bias_rows<FR>(kTcCodeBiasRows)),
+                                                                     num_sms(), &K.hdr->barrier, "render_kernel_tc_lerp", st);
+}
+template <int SAMPLER>
+static int launch_render_tc_lerp(const RenderKArgs &K, cudaStream_t st) {
+    return K.F.P.frame_table ? launch_render_tc_lerp_<SAMPLER, true>(K, st) : launch_render_tc_lerp_<SAMPLER, false>(K, st);
+}
+
+// The two render entry points share their checks and argument set-up; `lerp` selects render_kernel_tc_lerp.
+static int render_forward(const char *who, const bool lerp, const nsb_field_params *params, const nsb_field_opts *opts,
+                          const nsb_render_args *ra, void *stream) {
+    if (!params || !opts || !ra) { set_error("%s: null argument", who); return 1; }
     if (ra->n_rays <= 0) return 0;
-    if (check_field_params("nsb_render_forward", params)) return 1;
+    if (check_field_params(who, params)) return 1;
     const bool deform = opts->use_deformation != 0;
     if (!ra->origins || !ra->directions || !ra->t_starts || !ra->t_ends || !ra->ray_indices || !ra->sigma || !ra->rgb ||
         !ra->packed_info || !ra->out_rgb || !ra->out_acc || !ra->out_depth || !ra->workspace || (deform && !ra->offsets)) {
-        set_error("nsb_render_forward: null buffer");
+        set_error("%s: null buffer", who);
         return 1;
     }
-    if (!params->tables || !params->field_packed || !params->blend_codes) { set_error("nsb_render_forward: tables/field_packed/blend_codes missing"); return 1; }
+    if (!params->tables || !params->field_packed || !params->blend_codes) { set_error("%s: tables/field_packed/blend_codes missing", who); return 1; }
     if (deform && (!params->deform_packed_tb || !params->deform_bias || !params->deform_code_bias)) {
-        set_error("nsb_render_forward: deformation parameters missing");
+        set_error("%s: deformation parameters missing", who);
         return 1;
     }
-    if (ra->capacity <= 0) { set_error("nsb_render_forward: capacity <= 0"); return 1; }
+    if (ra->capacity <= 0) { set_error("%s: capacity <= 0", who); return 1; }
     if (ra->sampler == 0) {
-        if (ra->n_per_ray <= 0 || ra->capacity < ra->n_rays * (int64_t)ra->n_per_ray) { set_error("nsb_render_forward: capacity < n_rays * n_per_ray"); return 1; }
+        if (ra->n_per_ray <= 0 || ra->capacity < ra->n_rays * (int64_t)ra->n_per_ray) { set_error("%s: capacity < n_rays * n_per_ray", who); return 1; }
     } else if (ra->sampler == 1) {
-        if (!ra->near_planes || !ra->far_planes || !ra->binaries || !ra->aabbs) { set_error("nsb_render_forward: occupancy sampler arguments"); return 1; }
-        if (ra->levels < 1 || ra->levels > 8) { set_error("nsb_render_forward: levels must be in [1,8]"); return 1; }
-    } else { set_error("nsb_render_forward: unknown sampler"); return 1; }
+        if (!ra->near_planes || !ra->far_planes || !ra->binaries || !ra->aabbs) { set_error("%s: occupancy sampler arguments", who); return 1; }
+        if (ra->levels < 1 || ra->levels > 8) { set_error("%s: levels must be in [1,8]", who); return 1; }
+    } else { set_error("%s: unknown sampler", who); return 1; }
+    if (lerp) {
+        // the linear kernels are render_kernel_tc with the deformation MLP on wgmma; a frame table must be the stack of
+        // every timestep (one frame's table holds one timestep)
+        if (!deform) { set_error("%s: linear time needs the deformation field (use_deformation)", who); return 1; }
+        if (!params->deform_packed_umma) { set_error("%s: linear time needs the wgmma deformation weights (deform_packed_umma)", who); return 1; }
+        if (params->frame_table && params->frame_stride < params->levels.offset[NSB_MAX_LEVELS - 1] + (int64_t)params->levels.entries[NSB_MAX_LEVELS - 1]) {
+            set_error("%s: the frame table must be a timestep stack whose frame_stride covers every level's entries", who);
+            return 1;
+        }
+    }
     uint8_t *ws = reinterpret_cast<uint8_t *>(ra->workspace);
     RenderKArgs K;
     memset(&K, 0, sizeof(K));
@@ -1009,7 +1070,19 @@ extern "C" int nsb_render_forward(const nsb_field_params *params, const nsb_fiel
         // gather role of the field phase (tools/spill_report.py).
         const int rc = launch_march_occ_coop(K.M, K.packed_info, K.hdr, K.partials, K.capacity, ra->march_scratch, st);
         if (rc) return rc;
+        if (lerp) return launch_render_tc_lerp<2>(K, st);
         return deform ? launch_render<true, 2>(K, st) : launch_render<false, 2>(K, st);
     }
+    if (lerp) return launch_render_tc_lerp<4>(K, st);
     return deform ? launch_render<true, 0>(K, st) : launch_render<false, 0>(K, st);
+}
+}  // namespace nsb
+
+extern "C" int nsb_render_forward(const nsb_field_params *params, const nsb_field_opts *opts, const nsb_render_args *ra, void *stream) {
+    return render_forward("nsb_render_forward", false, params, opts, ra, stream);
+}
+
+extern "C" int nsb_render_forward_interp(const nsb_field_params *params, const nsb_field_opts *opts, const nsb_render_args *ra,
+                                         void *stream) {
+    return render_forward("nsb_render_forward_interp", true, params, opts, ra, stream);
 }

@@ -125,6 +125,30 @@ __device__ __forceinline__ BlendB make_blend_b(const nsb_field_opts &O, const fl
     return B;
 }
 
+// make_blend_b at a continuous time (DESIGN 4.2g): u = sample_time_u(t), the code row is time_lerp of the fp32 rows
+// floor(u) and floor(u) + 1 of `codes` [T][32], then folded and rounded to fp16 as above.
+__device__ __forceinline__ BlendB make_blend_b_lerp(const nsb_field_opts &O, const float *codes, float u, int n_timesteps,
+                                                    int lane) {
+    const int g = lane >> 2, q = lane & 3;
+    const int i0 = (int)u, i1 = min(i0 + 1, n_timesteps - 1);
+    const float lam = u - (float)i0;
+    const float4 *ra = reinterpret_cast<const float4 *>(codes + (size_t)i0 * NSB_MEMBERS) + 2 * q;
+    const float4 *rb = reinterpret_cast<const float4 *>(codes + (size_t)i1 * NSB_MEMBERS) + 2 * q;
+    const float4 a0 = __ldg(ra), a1 = __ldg(ra + 1), b0 = __ldg(rb), b1 = __ldg(rb + 1);
+    const float lo[4] = {time_lerp(a0.x, b0.x, lam), time_lerp(a0.y, b0.y, lam), time_lerp(a0.z, b0.z, lam), time_lerp(a0.w, b0.w, lam)};
+    const float hi[4] = {time_lerp(a1.x, b1.x, lam), time_lerp(a1.y, b1.y, lam), time_lerp(a1.z, b1.z, lam), time_lerp(a1.w, b1.w, lam)};
+    BlendB B;
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+        const float a = fmaf(lo[s], O.cw_scale[8 * q + s], O.cw_bias[8 * q + s]);
+        const float b = fmaf(hi[s], O.cw_scale[8 * q + 4 + s], O.cw_bias[8 * q + 4 + s]);
+        const uint32_t ha = __half_as_ushort(__float2half_rn(a)), hb = __half_as_ushort(__float2half_rn(b));
+        B.lo[s] = g == 0 ? ha : (g == 1 ? (ha << 16) : 0u);
+        B.hi[s] = g == 0 ? hb : (g == 1 ? (hb << 16) : 0u);
+    }
+    return B;
+}
+
 // One m-tile (2 levels) of loads for this lane's corner: 2 lines x 2 chunks of 16 B, plus the
 // lane's trilinear corner weights.
 struct GatherTile {

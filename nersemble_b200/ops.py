@@ -179,6 +179,40 @@ class NativeParams:
             self._stack = cached = (key, out)
         return cached[1]
 
+    def at_time(self, t: float) -> "NativeParams":
+        """A one-timestep view of the parameters at the continuous time t (DESIGN 4.2g): the tables and every weight are
+        shared with self; blend_codes [1,32] and deform_code_bias [1,2,128] are the time_lerp of the rows floor(u) and
+        floor(u) + 1, warp_codes [1,128] the fp16 of the interpolated fp32 codes (only the training backward reads it).
+        With T = 1 every kernel maps every sample to row 0, so any render, field or mesh call on the view answers at t.
+        At a snapped integer time the rows are the parent's row bit for bit.  Built on the device without a host
+        synchronisation; cached per (rows, lam, parameter versions)."""
+        i0, i1, lam = time_lerp(t, self.n_timesteps)
+        vers = tuple((x.data_ptr(), x._version) if x is not None else None
+                     for x in (self.blend_codes, self.deform_code_bias, self.warp_codes))
+        key = (i0, lam, vers)
+        cached = getattr(self, "_at_time", None)
+        if cached is None or cached[0] != key:
+            def rows(x):
+                if x is None:
+                    return None
+                a = x[i0:i0 + 1]
+                if lam == 0.0:
+                    return a.clone()
+                return _lerp_f32(a.float(), x[i1:i1 + 1].float(), lam).to(x.dtype)
+            if self.deform_packed_umma is None and getattr(self, "_umma_src", None) is not None:
+                self.deform_packed_umma = packing.pack_deform_umma_fast(*self._umma_src)     # shared, packed once
+            V = NativeParams(self.tables, self.deform_bias, self.field_packed, rows(self.warp_codes), rows(self.blend_codes),
+                             self.aabb, self.levels, 1)
+            V.field_packed_t, V.deform_packed_t, V.deform_packed_tb = self.field_packed_t, self.deform_packed_t, self.deform_packed_tb
+            V.deform_code_w, V.deform_code_bias = self.deform_code_w, rows(self.deform_code_bias)
+            V.deform_packed_umma, V.deform_packed_pe_t = self.deform_packed_umma, self.deform_packed_pe_t
+            if getattr(self, "_umma_src", None) is not None:
+                V._umma_src = self._umma_src
+            self._at_time = cached = (key, V)
+        V = cached[1]
+        V.tables = self.tables          # the plugin swaps in its current tables before every call
+        return V
+
     def pe_t(self) -> torch.Tensor:
         """packing.pack_deform_pe_t of the stem weights, packed on first use (only the deformation input gradient reads it)."""
         if self.deform_packed_pe_t is None:
@@ -220,6 +254,72 @@ class NativeParams:
                 p.levels.offset[l] = lv["offset"][l]
                 p.levels.hashed[l] = lv["hashed"][l]
         return p
+
+
+# Continuous time (DESIGN 4.2g).  "nearest" rounds a time to the nearest captured timestep, as the reference does;
+# "linear" interpolates the per-timestep codes between the two neighbouring timesteps.
+TIME_INTERPOLATIONS = ("nearest", "linear")
+TIME_SNAP = 2.0 ** -10      # timesteps: fp32 times k / (T - 1) land a few ulp off k (2.4e-4 timesteps at T = 2000)
+
+
+def time_lerp(t: float, n_timesteps: int):
+    """(i0, i1, lam) of time t over n_timesteps timesteps, in fp32 as the kernels form it (nsb_common.cuh
+    sample_time_u): u = clamp(t * (T - 1), 0, T - 1), snapped to rint(u) when within TIME_SNAP of it; i0 = floor(u),
+    i1 = min(i0 + 1, T - 1), lam = u - i0.  A per-timestep quantity q at t is fmaf(lam, q[i1] - q[i0], q[i0])."""
+    import numpy as np
+    T = int(n_timesteps)
+    if T < 1:
+        raise ValueError(f"time_lerp: n_timesteps must be >= 1, got {n_timesteps!r}")
+    tm = np.float32(T - 1)
+    with np.errstate(invalid="ignore", over="ignore"):
+        u = np.float32(np.float32(t) * tm)
+    u = np.float32(min(max(np.fmax(u, np.float32(0.0)), np.float32(0.0)), tm))     # fmaxf: NaN -> 0
+    r = np.float32(np.rint(u))
+    if abs(np.float32(u - r)) <= np.float32(TIME_SNAP):
+        u = r
+    i0 = min(int(np.floor(u)), T - 1)
+    return i0, min(i0 + 1, T - 1), float(np.float32(u - np.float32(i0)))
+
+
+def _lerp_f32(a: torch.Tensor, b: torch.Tensor, lam) -> torch.Tensor:
+    """fmaf(lam, b - a, a) in fp32 (lam a float or a tensor broadcasting against a): b - a rounded to fp32, then one
+    product and sum in fp64 (exact for the 24-bit lam times the 24-bit difference) and one rounding to fp32."""
+    lam = lam.double() if torch.is_tensor(lam) else float(lam)
+    return (a.double() + (b - a).double() * lam).float()
+
+
+def time_lerp_rows(times: torch.Tensor, n_timesteps: int):
+    """time_lerp of every time of a tensor, on its device: (i0 [n] int64, i1 [n] int64, lam [n] fp32)."""
+    T = int(n_timesteps)
+    t = times.detach().reshape(-1).to(_F32)
+    tm = float(T - 1)
+    u = torch.nan_to_num(t * tm, nan=0.0).clamp(0.0, tm)
+    r = torch.round(u)
+    u = torch.where((u - r).abs() <= TIME_SNAP, r, u)
+    i0 = u.floor().long().clamp(max=T - 1)
+    return i0, (i0 + 1).clamp(max=T - 1), u - i0.to(_F32)
+
+
+def time_codes(P: NativeParams, times: torch.Tensor) -> Dict[str, torch.Tensor]:
+    """Per-time interpolated codes for the per-sample-code kernels (field_forward(sample_blend_codes=,
+    sample_warp_codes=)), on the device without a host synchronisation: times [n] -> {"blend_codes" [n,32] fp32,
+    "warp_codes" [n,128] fp32 (with a deformation field)}, each time_lerp of the parameters' rows."""
+    i0, i1, lam = time_lerp_rows(times, P.n_timesteps)
+    lam = lam[:, None]
+    out = {}
+    if P.blend_codes is not None:
+        out["blend_codes"] = _lerp_f32(P.blend_codes[i0], P.blend_codes[i1], lam)
+    if P.warp_codes is not None:
+        wc = P.warp_codes.float()
+        out["warp_codes"] = _lerp_f32(wc[i0], wc[i1], lam)
+    return out
+
+
+def _check_time_interpolation(time_interpolation, who: str) -> bool:
+    """True for "linear"; ValueError for anything not in TIME_INTERPOLATIONS."""
+    if time_interpolation not in TIME_INTERPOLATIONS:
+        raise ValueError(f"{who}: time_interpolation must be one of {TIME_INTERPOLATIONS}, got {time_interpolation!r}")
+    return time_interpolation == "linear"
 
 
 def make_opts(window_hash: Optional[float], window_deform: Optional[float], use_deformation: bool,
@@ -1126,7 +1226,8 @@ def render_rays(P: NativeParams, origins, directions, ray_times, *, window_hash=
                 step: float = 1e-3, cone_angle: float = 0.0, capacity: Optional[int] = None,
                 disable_initial=True, soft_transition=True, single_traversal: bool = True,
                 uniform_time: Optional[float] = None, line_gather: bool = False,
-                want_normals: bool = False, normals_space: str = "canonical") -> RenderResult:
+                want_normals: bool = False, normals_space: str = "canonical",
+                time_interpolation: str = "nearest") -> RenderResult:
     """The fused inference render (nsb_render_forward): sampler -> field -> composite without a host synchronisation.
     sampler 'fixed' (n_per_ray steps from the box entry: ONE launch) or 'occupancy' (nerfacc march of `binaries`
     [levels,res,res,res] within per-ray near_planes / far_planes: the cooperative march launch + one fused launch;
@@ -1138,9 +1239,24 @@ def render_rays(P: NativeParams, origins, directions, ray_times, *, window_hash=
     want_normals=True adds `normals` [R,3]: the world-space surface normals of the call's own packed samples (field_normals
     on the same tables), composited with the render weights and normalised; still without a host synchronisation.
     normals_space="observation" applies the deformation Jacobian to them (field_normals(space=...)); without
-    use_deformation both spaces are the same."""
+    use_deformation both spaces are the same.
+    time_interpolation="linear" renders at continuous times (DESIGN 4.2g) instead of rounding each time to the nearest
+    timestep: with a uniform_time on the one-timestep view P.at_time(uniform_time) (any sampler, deformation and
+    normals); with mixed ray_times on nsb_render_forward_interp (timestep stack or line gather, chosen as above), which
+    needs use_deformation, the wgmma kernels and no normals.  Neither path synchronises with the host."""
     if normals_space not in NORMAL_SPACES:
         raise ValueError(f"normals_space must be one of {NORMAL_SPACES}, got {normals_space!r}")
+    # the default ("nearest") costs one comparison: the host issues this call back to back in the render loop
+    mixed_linear = (time_interpolation != "nearest" and _check_time_interpolation(time_interpolation, "render_rays")
+                    and uniform_time is None)
+    if mixed_linear:
+        why = ("use_deformation=False" if not use_deformation else "want_normals=True" if want_normals else
+               "the non-wgmma kernels (NSB_TCGEN05=0)" if (P.deform_packed_umma is None and getattr(P, "_umma_src", None) is None)
+               else None)
+        if why is not None:
+            raise NotImplementedError(f"render_rays: time_interpolation='linear' with mixed ray times and {why}")
+    elif time_interpolation == "linear":
+        P = P.at_time(uniform_time)
     lib = _lib.load()
     origins, directions = _f32c(origins).reshape(-1, 3), _f32c(directions).reshape(-1, 3)
     ray_times = None if ray_times is None else _f32c(ray_times).reshape(-1)
@@ -1204,7 +1320,10 @@ def render_rays(P: NativeParams, origins, directions, ray_times, *, window_hash=
     if use_deformation:
         frame = _blended_tables(P, uniform_time, window_hash, disable_initial, soft_transition, line_gather)
     cp = P.c_params(inference=True, frame=frame)
-    _lib.check(lib.nsb_render_forward(C.byref(cp), C.byref(opts), C.byref(a), _stream()), "nsb_render_forward")
+    if mixed_linear:
+        _lib.check(lib.nsb_render_forward_interp(C.byref(cp), C.byref(opts), C.byref(a), _stream()), "nsb_render_forward_interp")
+    else:
+        _lib.check(lib.nsb_render_forward(C.byref(cp), C.byref(opts), C.byref(a), _stream()), "nsb_render_forward")
     if want_normals:
         # the pass reads the packed samples the render left in `buf`; their count stays on the device (header n_total)
         s = _lib.Samples()
@@ -1514,11 +1633,14 @@ def extract_mesh_sequence(P: NativeParams, *, times: Sequence[float], reference_
 
 def render_packed(P: NativeParams, origins, directions, ray_times, t_starts, t_ends, ray_indices, packed_info, *,
                   window_hash=None, window_deform=None, use_deformation=True, training=False,
-                  disable_initial=True, soft_transition=True) -> Dict[str, torch.Tensor]:
-    """NeRSembleNGPModel.get_outputs after the sampler (nersemble_instant_ngp.py:297-364)."""
+                  disable_initial=True, soft_transition=True, sample_blend_codes=None,
+                  sample_warp_codes=None) -> Dict[str, torch.Tensor]:
+    """NeRSembleNGPModel.get_outputs after the sampler (nersemble_instant_ngp.py:297-364).  sample_blend_codes [n,32] /
+    sample_warp_codes [n,128]: per-sample codes instead of the rows of the ray times (field_forward)."""
     f = field_forward(P, window_hash=window_hash, window_deform=window_deform, use_deformation=use_deformation,
                       origins=origins, directions=directions, ray_times=ray_times, t_starts=t_starts, t_ends=t_ends,
-                      ray_indices=ray_indices, want=("sigma", "rgb", "offsets"),
+                      ray_indices=ray_indices, want=("sigma", "rgb", "offsets"), sample_blend_codes=sample_blend_codes,
+                      sample_warp_codes=sample_warp_codes if use_deformation else None,
                       disable_initial=disable_initial, soft_transition=soft_transition)
     c = composite(packed_info, t_starts, t_ends, f["sigma"], f["rgb"], f["offsets"] if use_deformation else None,
                   training=training)

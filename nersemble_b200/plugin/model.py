@@ -205,6 +205,9 @@ class NeRSembleNGPModel(Model):
                                          # surface normals composited with the render weights (unit vectors, [R,3] / [H,W,3])
         self.render_normals_space = "canonical"  # "observation": the normals of the observed (deformed) surface, with the
                                          # deformation Jacobian applied; "canonical": of the canonical surface the field stores
+        self.time_interpolation = "nearest"  # eval renders: "nearest" rounds a ray's time to the nearest timestep (the
+                                         # reference); "linear" interpolates the time codes between the two neighbouring
+                                         # timesteps (DESIGN 4.2g).  Training always rounds.
 
     def populate_modules(self):
         """models/nersemble_instant_ngp.py:81-179 (+ BaseModel.populate_modules, base.py:38-47)."""
@@ -354,6 +357,11 @@ class NeRSembleNGPModel(Model):
         camera = None if intrinsics is None else ops._flow_camera((intrinsics, camera_to_world), "render_flow")
         n = self.config.eval_num_rays_per_chunk
         h, w = camera_ray_bundle.origins.shape[:2]
+        if self._linear_time():
+            # the inverse deformation runs at the timesteps' own codes; interpolated ones are not supported
+            lam = ops.time_lerp_rows(self._ray_times(camera_ray_bundle), self.config.n_timesteps)[2]
+            if bool((lam != 0).any()):
+                raise NotImplementedError("render_flow: time_interpolation='linear' with a frame time between timesteps")
         uniform_time = self._frame_uniform_time(camera_ray_bundle)
         _, wd = self._windows()
         lists: Dict[str, list] = {}
@@ -438,6 +446,18 @@ class NeRSembleNGPModel(Model):
             return ray_bundle.times.reshape(-1).float()
         return ray_bundle.metadata['timesteps'].reshape(-1).float() / max(self.config.n_timesteps - 1, 1)
 
+    def _linear_time(self) -> bool:
+        return self.time_interpolation != "nearest" and ops._check_time_interpolation(
+            self.time_interpolation, "NeRSembleNGPModel.time_interpolation")
+
+    def _linear_mixed_fused(self) -> bool:
+        """time_interpolation "linear" on a bundle of mixed times: whether the fused linear kernels apply (deformation field
+        on the wgmma kernels); otherwise get_outputs evaluates the field with per-sample interpolated codes."""
+        if self.render_normals:
+            raise NotImplementedError("time_interpolation='linear' with render_normals on rays of mixed times")
+        P = self.native_params()
+        return self.config.use_deformation_field and (P.deform_packed_umma is not None or getattr(P, "_umma_src", None) is not None)
+
     def _fused_render(self, ray_bundle: RayBundle, uniform_time: Optional[float] = None) -> "ops.RenderResult":
         """Eval render of a (flat) ray bundle through nsb_render_forward: the nerfacc occupancy march as one cooperative
         launch + field and compositing fused into one launch; the packed sample count stays on the device.
@@ -452,7 +472,8 @@ class NeRSembleNGPModel(Model):
                                near_planes=near_planes, far_planes=far_planes, binaries=og.binaries, aabbs=og.aabbs,
                                step=cfg.render_step_size, cone_angle=cfg.cone_angle, uniform_time=uniform_time,
                                line_gather=not self.frame_tables, want_normals=self.render_normals,
-                               normals_space=self.render_normals_space, **self._blend_opts())
+                               normals_space=self.render_normals_space, time_interpolation=self.time_interpolation,
+                               **self._blend_opts())
 
     @torch.no_grad()
     def _packed_normals(self, ray_bundle: RayBundle, ray_times, starts, ends, ray_indices, packed_info, weights, offsets,
@@ -529,10 +550,12 @@ class NeRSembleNGPModel(Model):
         n = self.config.eval_num_rays_per_chunk
         h, w = camera_ray_bundle.origins.shape[:2]
         uniform_time = self._frame_uniform_time(camera_ray_bundle)
+        # linear time, mixed times and no fused linear kernel: get_outputs' per-sample-code path, chunk by chunk
+        general = self._linear_time() and uniform_time is None and not self._linear_mixed_fused()
         lists: Dict[str, list] = {}
         for i in range(0, h * w, n):
             rb = camera_ray_bundle.get_row_major_sliced_ray_bundle(i, i + n)
-            res = self._fused_render(rb, uniform_time)
+            res = self.get_outputs(rb) if general else self._fused_render(rb, uniform_time)
             for name in ("rgb", "accumulation", "depth", "num_samples_per_ray", "deformation", "normals"):
                 if name in res:
                     lists.setdefault(name, []).append(res[name])
@@ -545,7 +568,11 @@ class NeRSembleNGPModel(Model):
         num_rays = len(ray_bundle)
         # the differentiable path is the TRAINING path (training-mode compositing); eval renders are inference-only
         needs_grad = self.training and torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())
-        if not needs_grad and self._fused_ok() and jitter is None:
+        linear = self._linear_time()
+        if linear and needs_grad:
+            raise ValueError("time_interpolation='linear' is for eval renders; training rounds ray times to the nearest "
+                             "timestep (set time_interpolation='nearest')")
+        if not needs_grad and self._fused_ok() and jitter is None and not (linear and not self._linear_mixed_fused()):
             # eval: fused render; ONE host synchronisation (the packed sample count) to hand out exact-size per-sample tensors
             res = self._fused_render(ray_bundle)
             pk = res.packed()
@@ -610,9 +637,19 @@ class NeRSembleNGPModel(Model):
                 outputs["normals"] = self._packed_normals(ray_bundle, ray_times, starts, ends, ray_indices, packed_info,
                                                           weights, res[5] if cfg.use_deformation_field else None, True)
             return outputs
+        codes = {}
+        if linear:      # per-sample interpolated codes into the per-sample-code kernels (DESIGN 4.2g)
+            if self.render_normals:
+                raise NotImplementedError("time_interpolation='linear' with render_normals on rays of mixed times")
+            tc = ops.time_codes(self.native_params(), ray_times)
+            ri = ray_indices.long()
+            codes["sample_blend_codes"] = tc["blend_codes"][ri].contiguous()
+            if "warp_codes" in tc and cfg.use_deformation_field:
+                codes["sample_warp_codes"] = tc["warp_codes"][ri].contiguous()
         out = ops.render_packed(self.native_params(), ray_bundle.origins, ray_bundle.directions, ray_times, starts, ends,
                                 ray_indices, packed_info, window_hash=wh, window_deform=wd,
-                                use_deformation=cfg.use_deformation_field, training=self.training, **self._blend_opts())
+                                use_deformation=cfg.use_deformation_field, training=self.training, **codes,
+                                **self._blend_opts())
         if cfg.use_deformation_field:
             ray_samples.frustums.set_offsets(out["offsets"])
         outputs = {

@@ -5,7 +5,8 @@ backward, rank-1 expand + fused Adam, occupancy update, component kernels, surfa
 space), the deformation input gradient (ragged last tile, a device sample count below the buffer size), the mesh export
 (a ragged last tile of grid points, an occupancy grid, vertex normals and colours), the deformation Jacobian and inverse
 (ragged last tile, several tiles per CTA, per-sample warp codes), a tracked mesh sequence, and the flow pass (selection
-of a fixed-stride render, the inverse over the device-side selected count, compositing with a camera)."""
+of a fixed-stride render, the inverse over the device-side selected count, compositing with a camera), and renders
+between timesteps on both gathers."""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
@@ -55,6 +56,9 @@ rf = ops.render_rays(P, o, d, t, window_hash=32.0, window_deform=7.0, sampler="f
                      step=bench.STEP)
 ops.render_flow(P, rf, o, d, t, time_to=0.75, window_deform=7.0, camera=cam, max_iter=5)
 ops.render_flow(P, rf, o, d, t, time_to=0.0, window_deform=7.0)
+for lg in (False, True):        # renders between timesteps (nsb_render_forward_interp): timestep stack and line gather
+    ops.render_rays(P, o, d, t, window_hash=32.0, window_deform=7.0, sampler="fixed", n_per_ray=100, near_plane=bench.NEAR,
+                    step=bench.STEP, line_gather=lg, time_interpolation="linear")
 # plugin model: occupancy march + pre-pass + training step + occupancy update
 m = bench.build_model(S, dev).train()
 occ = bench.blob_occupancy(seed=5)
